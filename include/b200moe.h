@@ -19,7 +19,9 @@
  *   GateLinear.forward (router GEMM) ...... vllm/model_executor/layers/fused_moe/router/gate_linear.py:171-221
  *   _moe_C.moe_permute / moe_unpermute .... csrc/libtorch_stable/moe/moe_permute_unpermute_op.cu:59-207
  *   _C.sm100_cutlass_mla_decode ........... csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262
- *   paged GQA decode (FlashInfer backend) . vllm/v1/attention/backends/flashinfer.py (cache layout :398-409)
+ *   paged GQA decode (FlashInfer backend) . vllm/v1/attention/backends/flashinfer.py (cache layout :398-433, K / V views
+ *                                           :2276-2290)
+ *   fused_qk_norm_rope + reshape_and_cache_flash .. vllm/_custom_ops.py:279, csrc/libtorch_stable/cache_kernels.cu:315-400
  */
 #ifndef B200MOE_H_
 #define B200MOE_H_
@@ -206,13 +208,48 @@ int b200_mla_decode_vup(void* stream, const void* q_nope, const void* q_pe, int 
                         float descale_q, float descale_k, const int32_t* seq_lens, const int32_t* page_table, int batch,
                         int num_heads, int page_size, int max_pages, float sm_scale, int num_splits, void* workspace,
                         const void* w_uv, void* out_v, void* out_latent, float* lse);
-/* Paged GQA decode.  q [B,Hq,D] bf16, k_cache/v_cache [num_pages,page_size,Hkv,D] bf16, D=128;
+/* Paged GQA decode.  q [B,Hq,D] bf16, k_cache/v_cache [num_pages,page_size,Hkv,D] bf16 (contiguous), D=128;
  * out bf16 [B,Hq,D], lse f32 [B,Hq] or NULL. */
 int64_t b200_gqa_decode_workspace_bytes(int batch, int num_q_heads, int head_dim, int num_splits);
 int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void* v_cache,
                     const int32_t* seq_lens, const int32_t* page_table, int batch, int num_q_heads,
                     int num_kv_heads, int head_dim, int page_size, int max_pages, float sm_scale,
                     int num_splits, void* workspace, void* out, float* lse);
+/* Same on caches described by base pointer + strides in elements: row (page, slot, kv head) of a cache starts at
+ * page * block_stride + slot * page_stride + head * head_stride, its D elements contiguous.  This reads the FlashInfer
+ * backend's cache in place: one tensor per layer, logical (blocks, Hkv, page, 2D), NHD (blocks, page, Hkv, 2D) or HND
+ * in memory (flashinfer.py:398-433), handed out as kv_cache.transpose(1, 2).split(D, -1) (flashinfer.py:2276-2290),
+ * i.e. k_cache = base, v_cache = base + D with the tensor's own strides.  b200_gqa_decode passes the contiguous strides
+ * (page_size*Hkv*D, Hkv*D, D).  Strides must be positive multiples of 8 elements and the cache pointers 16-byte aligned
+ * (16-byte cp.async rows); B200_ERR_INVALID otherwise. */
+int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const void* v_cache, int64_t block_stride,
+                       int64_t page_stride, int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table,
+                       int batch, int num_q_heads, int num_kv_heads, int head_dim, int page_size, int max_pages,
+                       float sm_scale, int num_splits, void* workspace, void* out, float* lse);
+/* The GQA decode kernel's neighbour, bf16: one launch per step for what the reference runs as Qwen3's per-head q/k RMSNorm
+ * (models/qwen3_moe.py:333-351) + RoPE (fused_qk_norm_rope, vllm/_custom_ops.py:279; rotary_embedding/base.py:161-201)
+ * + reshape_and_cache_flash (csrc/libtorch_stable/cache_kernels.cu:315-400, called at flashinfer.py:2276-2290).
+ *   qkv           [T, (Hq + 2 Hkv) * D] bf16, contiguous: the fused QKV projection's output (q heads, k heads, v heads);
+ *   q_weight / k_weight  bf16 [D] RMSNorm weights, or NULL to skip that norm (Mixtral); eps its epsilon.  The norm is
+ *                 vllm/ir/ops/layernorm.py:10-21 in its order: fp32 statistics, rounded to bf16, times the weight with one
+ *                 rounding;
+ *   cos_sin_cache bf16 [max_position, rotary_dim] = cos | sin (RotaryEmbedding._match_cos_sin_cache_dtype); rotary_dim
+ *                 even, <= D; is_neox 1 = NeoX halves (p, p + rotary_dim/2), 0 = GPT-J pairs (2p, 2p + 1).  positions
+ *                 (i64 [T]) are CLAMPED to [0, max_position): the table is never read outside its rows.  RoPE is computed
+ *                 in fp32 from the bf16 inputs and rounded once (<= 2 bf16 ulp from forward_static's bf16 arithmetic);
+ *   q_out         [T, Hq, D] bf16, contiguous: the rotated q, b200_gqa_decode's q;
+ *   k_cache / v_cache  base pointers + block_stride / page_stride / head_stride (elements) as b200_gqa_decode_ex takes them
+ *                 (= what reshape_and_cache_flash is given: NHD / HND packed views or separate caches); page_size = block
+ *                 size.  Row slot_mapping[t] (i64, slot = block * page_size + offset; < 0 = padded token, nothing
+ *                 written) of every kv head <- rotated k / the untouched v.
+ * D = head_dim must be 128; strides positive multiples of 8 elements, pointers 16-byte aligned; NULL only for the weights.
+ * B200_ERR_INVALID otherwise. */
+int b200_gqa_qknorm_rope_cache_write(void* stream, const void* qkv, const int64_t* positions, const void* cos_sin_cache,
+                                     int max_position, int rotary_dim, int is_neox, const void* q_weight,
+                                     const void* k_weight, float eps, const int64_t* slot_mapping, void* k_cache,
+                                     void* v_cache, int64_t block_stride, int64_t page_stride, int64_t head_stride,
+                                     int page_size, void* q_out, int num_tokens, int num_heads, int num_kv_heads,
+                                     int head_dim);
 
 /* ---- expert-parallel exchange over NVLink peer memory ---------------------------------------------- */
 /* Sum-combine of per-rank partial MoE outputs through peer-mapped buffers (the lk_moe EP/TP contract:

@@ -1,7 +1,8 @@
 // Paged decode attention (one query token per request), split-KV + LSE merge.
 //   MLA (absorbed): q = [q_nope(512) | q_pe(64)], one shared latent KV head, K = all 576 cols, V = first 512
 //                   (op contract of reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262)
-//   GQA           : q [B,Hq,D], separate K / V caches [pages,page,Hkv,D]
+//   GQA           : q [B,Hq,D], K / V caches [pages,page,Hkv,D] given by base pointer + (page, slot, head) strides:
+//                   separate contiguous caches or the halves of the FlashInfer backend's packed NHD / HND cache
 //                   (reference tests/kernels/attention/test_flashinfer.py:29-80)
 //
 // v1 kernel (CUDA cores): a CTA owns (request, kv-head, head-group, split); KV tiles of TOK tokens are staged
@@ -28,8 +29,10 @@ __global__ void __launch_bounds__(WARPS * 32)
                        const __nv_bfloat16* __restrict__ kc, const __nv_bfloat16* __restrict__ vc,
                        const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ page_table, int Hq, int Hkv,
                        int page_size, int max_pages, float scale_log2, int num_splits, float* __restrict__ part_o,
-                       float* __restrict__ part_ml) {
+                       float* __restrict__ part_ml, int64_t block_stride, int64_t page_stride, int64_t head_stride) {
   // blockIdx.x = ((b * Hkv + hkv) * groups_per_kv + hg), blockIdx.y = split
+  // GQA: K / V row of (page, slot in page, kv head) at page * block_stride + slot * page_stride + hkv * head_stride
+  // (elements); MLA: the latent cache is contiguous and the strides are unused
   const int G = Hq / Hkv;
   const int groups_per_kv = (G + WARPS - 1) / WARPS;
   int bx = blockIdx.x;
@@ -81,7 +84,8 @@ __global__ void __launch_bounds__(WARPS * 32)
         const int tok = t0 + tt;
         const int page = page_table[(size_t)b * max_pages + tok / page_size];
         const size_t row = (size_t)page * page_size + tok % page_size;
-        const __nv_bfloat16* src = MLA ? kc + row * DK : kc + (row * Hkv + hkv) * DK;
+        const __nv_bfloat16* src =
+            MLA ? kc + row * DK : kc + page * block_stride + (tok % page_size) * page_stride + hkv * head_stride;
         *reinterpret_cast<uint4*>(&ks[tt][c * 8]) = *reinterpret_cast<const uint4*>(src + c * 8);
       }
     }
@@ -92,9 +96,8 @@ __global__ void __launch_bounds__(WARPS * 32)
         if (tt < nt) {
           const int tok = t0 + tt;
           const int page = page_table[(size_t)b * max_pages + tok / page_size];
-          const size_t row = (size_t)page * page_size + tok % page_size;
-          *reinterpret_cast<uint4*>(&vs[MLA ? 0 : tt][c * 8]) =
-              *reinterpret_cast<const uint4*>(vc + (row * Hkv + hkv) * DV + c * 8);
+          *reinterpret_cast<uint4*>(&vs[MLA ? 0 : tt][c * 8]) = *reinterpret_cast<const uint4*>(
+              vc + page * block_stride + (tok % page_size) * page_stride + hkv * head_stride + c * 8);
         }
       }
     }
@@ -289,7 +292,7 @@ int b200_mla_decode_ex(void* stream, const void* q_nope, const void* q_pe, int q
   decode_attn_kernel<576, 512, WARPS, true><<<grid, WARPS * 32, 0, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(q_nope), reinterpret_cast<const __nv_bfloat16*>(q_pe),
       reinterpret_cast<const __nv_bfloat16*>(kv_cache), nullptr, seq_lens, page_table, num_heads, 1, page_size,
-      max_pages, sm_scale * 1.4426950408889634f, num_splits, po, pml);
+      max_pages, sm_scale * 1.4426950408889634f, num_splits, po, pml, 0, 0, 0);
   decode_merge_kernel<512><<<(batch * num_heads + 3) / 4, 128, 0, st>>>(po, pml, batch * num_heads, num_splits,
                                                                        reinterpret_cast<__nv_bfloat16*>(out), lse);
   g_launches += 2;
@@ -302,6 +305,15 @@ int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void
                     const int32_t* page_table, int batch, int num_q_heads, int num_kv_heads, int head_dim,
                     int page_size, int max_pages, float sm_scale, int num_splits, void* workspace, void* out,
                     float* lse) {
+  const int64_t hs = head_dim, ps = (int64_t)num_kv_heads * head_dim, bs = (int64_t)page_size * num_kv_heads * head_dim;
+  return b200_gqa_decode_ex(stream, q, k_cache, v_cache, bs, ps, hs, seq_lens, page_table, batch, num_q_heads,
+                            num_kv_heads, head_dim, page_size, max_pages, sm_scale, num_splits, workspace, out, lse);
+}
+
+int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const void* v_cache, int64_t block_stride,
+                       int64_t page_stride, int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table,
+                       int batch, int num_q_heads, int num_kv_heads, int head_dim, int page_size, int max_pages,
+                       float sm_scale, int num_splits, void* workspace, void* out, float* lse) {
   if (!q || !k_cache || !v_cache || !seq_lens || !page_table || !workspace || !out || batch <= 0 ||
       num_q_heads <= 0 || num_kv_heads <= 0 || num_q_heads % num_kv_heads || page_size <= 0 || num_splits <= 0) {
     set_error("b200_gqa_decode: bad argument");
@@ -309,6 +321,12 @@ int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void
   }
   if (head_dim != 128) {
     set_error("b200_gqa_decode: head_dim must be 128");
+    return B200_ERR_INVALID;
+  }
+  // 16-byte cp.async / vector loads of every K / V row: strides in multiples of 8 elements, 16-byte aligned bases
+  if (block_stride <= 0 || page_stride <= 0 || head_stride <= 0 || block_stride % 8 || page_stride % 8 || head_stride % 8 ||
+      (reinterpret_cast<uintptr_t>(k_cache) | reinterpret_cast<uintptr_t>(v_cache)) % 16) {
+    set_error("b200_gqa_decode: cache strides must be positive multiples of 8 elements, cache pointers 16-byte aligned");
     return B200_ERR_INVALID;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -323,8 +341,8 @@ int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void
     return !(v && v[0] == '1');
   }();
   if (use_tc && G <= 128 && num_splits <= 1024 && (int64_t)num_splits * 128 >= (int64_t)max_pages * page_size) {
-    const int rc = launch_gqa_tc(st, q, k_cache, v_cache, seq_lens, page_table, batch, num_q_heads, num_kv_heads,
-                                 page_size, max_pages, sm_scale, num_splits, po, pml, out, lse);
+    const int rc = launch_gqa_tc(st, q, k_cache, v_cache, block_stride, page_stride, head_stride, seq_lens, page_table, batch,
+                                 num_q_heads, num_kv_heads, page_size, max_pages, sm_scale, num_splits, po, pml, out, lse);
     if (rc <= 0) return rc;   // rc == 1: more work items per CTA than the kernel's table holds
   }
 #define LAUNCH_GQA(W)                                                                                          \
@@ -334,7 +352,7 @@ int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void
     decode_attn_kernel<128, 128, W, false><<<grid, W * 32, 0, st>>>(                                           \
         reinterpret_cast<const __nv_bfloat16*>(q), nullptr, reinterpret_cast<const __nv_bfloat16*>(k_cache),   \
         reinterpret_cast<const __nv_bfloat16*>(v_cache), seq_lens, page_table, num_q_heads, num_kv_heads,      \
-        page_size, max_pages, sl2, num_splits, po, pml);                                                       \
+        page_size, max_pages, sl2, num_splits, po, pml, block_stride, page_stride, head_stride);               \
   }
   if (G <= 4)
     LAUNCH_GQA(4)

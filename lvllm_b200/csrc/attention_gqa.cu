@@ -8,7 +8,8 @@
 //   O^T[128 dims, N]    = V^T[128 dims, 128 tokens] . P^T          (A = V tile read MN-major; B = P rows, K-major)
 //   L[128, N]           = 1[128, 128 tokens] . P^T                 (row sums of P on the tensor core: every
 //                                                                   epilogue thread reads l[h] from its own lane)
-// K and V tiles are gathered with cp.async straight into 128B-swizzled [64-dim block][128 tokens][128 B] blocks;
+// K and V tiles are gathered with cp.async straight into 128B-swizzled [64-dim block][128 tokens][128 B] blocks; a row is
+// found through (page, slot, head) strides, so the K / V halves of a packed NHD / HND cache are read in place;
 // NST stages of (Q, K, V) let the loaders run ahead of the MMAs; the accumulators cross from the MMA warpgroup to the
 // softmax / epilogue threads through the exchange area (common.cuh), S^T double-buffered so that QK^T of item n+1
 // overlaps softmax of item n.  Partial (O, m, l) per split are merged by attn_merge_kernel.
@@ -62,6 +63,7 @@ template <int N>
 __global__ void __launch_bounds__(GQA_THREADS, 1)
     gqa_decode_tc_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
                          const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ seq_lens,
+                         int64_t block_stride, int64_t page_stride, int64_t head_stride,
                          const int32_t* __restrict__ page_table, int B, int Hq, int Hkv, int page_size, int max_pages,
                          float scale_log2, int num_splits, int NST, float* __restrict__ part_o,
                          float* __restrict__ part_ml) {
@@ -139,11 +141,11 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
           cp_async16(q_t + sw128_offset(r, c * 16), src, qok);
           cp_async16(q_t + qbytes + sw128_offset(r, c * 16), src + 64, qok);
         }
-        size_t rowoff[8];
+        int64_t rowoff[8];   // cache element offsets (strides in elements: packed K|V views or separate caches)
 #pragma unroll
         for (int u = 0; u < 8; ++u) {
           const int tok = split * GQA_TOK + r0 + 16 * u;
-          rowoff[u] = (((size_t)pg[u] * page_size + tok % page_size) * Hkv + kvh) * 128 + c * 8;
+          rowoff[u] = pg[u] * block_stride + (tok % page_size) * page_stride + kvh * head_stride + c * 8;
         }
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb) {
@@ -379,9 +381,10 @@ __global__ void __launch_bounds__(DV / 4) attn_merge_kernel(const float* __restr
   if (lse && tid == 0) lse[w] = (lsum > 0.f) ? (mx * 0.6931471805599453f + logf(lsum)) : -CUDART_INF_F;
 }
 
-int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc, const int32_t* seq_lens,
-                  const int32_t* page_table, int batch, int Hq, int Hkv, int page_size, int max_pages, float sm_scale,
-                  int num_splits, float* part_o, float* part_ml, void* out, float* lse) {
+int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc, int64_t block_stride, int64_t page_stride,
+                  int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table, int batch, int Hq, int Hkv,
+                  int page_size, int max_pages, float sm_scale, int num_splits, float* part_o, float* part_ml, void* out,
+                  float* lse) {
   static bool attr = false;
   static int num_sms = 0;
   if (!attr) {
@@ -418,7 +421,7 @@ int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc
   auto kern = N == 16 ? gqa_decode_tc_kernel<16> : gqa_decode_tc_kernel<32>;
   kern<<<grid, GQA_THREADS, smem, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(kc),
-      reinterpret_cast<const __nv_bfloat16*>(vc), seq_lens, page_table, batch, Hq, Hkv, page_size, max_pages,
+      reinterpret_cast<const __nv_bfloat16*>(vc), seq_lens, block_stride, page_stride, head_stride, page_table, batch, Hq, Hkv, page_size, max_pages,
       sm_scale * 1.4426950408889634f, num_splits, nst, part_o, part_ml);
   attn_merge_kernel<128><<<batch * Hq, 32, 0, st>>>(part_o, part_ml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
   g_launches += 2;

@@ -252,15 +252,37 @@ def mla_q_absorb(q_nope: torch.Tensor, w_uk_t: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def _kv_cache_strides(k_cache: torch.Tensor, v_cache: torch.Tensor) -> tuple[int, int, int]:
+    """(block, page, head) strides in elements of a pair of [blocks, page, Hkv, 128] bf16 cache views, checked against what
+    the kernels address: the FlashInfer backend's packed NHD / HND halves (kv_cache.transpose(1, 2).split(128, -1),
+    flashinfer.py:2276-2290) or separate contiguous caches.  Never copies: a write through a copy would be lost."""
+    for t, n in ((k_cache, "k_cache"), (v_cache, "v_cache")):
+        if not t.is_cuda:
+            raise ValueError(f"{n} must be a CUDA tensor (lvllm_b200 has no CPU path)")
+        if t.dtype != torch.bfloat16 or t.dim() != 4 or t.shape[-1] != 128:
+            raise ValueError(f"{n} must be a bf16 [blocks, page, num_kv_heads, 128] view, got {t.dtype} {tuple(t.shape)}")
+    if k_cache.shape != v_cache.shape or k_cache.stride() != v_cache.stride() or k_cache.device != v_cache.device:
+        raise ValueError("k_cache and v_cache must be views of the same shape and strides on one device")
+    st = k_cache.stride()
+    if st[3] != 1 or any(x <= 0 or x % 8 for x in st[:3]) or k_cache.data_ptr() % 16 or v_cache.data_ptr() % 16:
+        raise ValueError(f"cache views need a contiguous head dim, strides in positive multiples of 8 elements and "
+                         f"16-byte aligned bases (16-byte row loads), got strides {st}")
+    return st[0], st[1], st[2]
+
+
 def gqa_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, seq_lens: torch.Tensor,
                page_table: torch.Tensor, sm_scale: float, num_kv_splits: int = 0, max_seq_len: int | None = None):
-    """Paged GQA decode (q [B,Hq,128] bf16; caches [pages,page,Hkv,128] bf16).  Returns (out, lse).
+    """Paged GQA decode (q [B,Hq,128] bf16; caches [pages,page,Hkv,128] bf16 views).  Returns (out, lse).
+    The caches are read in place through their own strides: separate contiguous caches, or the K / V halves of the
+    FlashInfer backend's packed NHD / HND cache exactly as the backend hands them out (kv_cache.transpose(1, 2)
+    .split(128, -1)); the head dim must be contiguous and the other strides multiples of 8 elements (ValueError otherwise).
     ``max_seq_len`` (host-side bound on seq_lens, as the reference's attention metadata carries it) sizes the split count
     and the B*Hq*splits*130*4-byte workspace from the real context instead of the page-table width (= max_model_len)."""
-    qq, kc, vc = _cuda(q, "q"), _cuda(k_cache, "k_cache"), _cuda(v_cache, "v_cache")
-    assert qq.dtype == torch.bfloat16 and kc.dtype == torch.bfloat16
+    qq = _cuda(q, "q")
+    assert qq.dtype == torch.bfloat16
+    bstride, pstride, hstride = _kv_cache_strides(k_cache, v_cache)
     B, Hq, D = qq.shape
-    page, Hkv = kc.shape[1], kc.shape[2]
+    page, Hkv = k_cache.shape[1], k_cache.shape[2]
     sl = _cuda(seq_lens.to(torch.int32), "seq_lens")
     pt = _cuda(page_table.to(torch.int32), "page_table")
     if max_seq_len is not None:
@@ -275,8 +297,51 @@ def gqa_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, se
     ws = torch.empty(L.lib().b200_gqa_decode_workspace_bytes(B, Hq, D, num_kv_splits), dtype=torch.uint8, device=qq.device)
     out = torch.empty(B, Hq, D, dtype=torch.bfloat16, device=qq.device)
     lse = torch.empty(B, Hq, dtype=torch.float32, device=qq.device)
-    rc = L.lib().b200_gqa_decode(_stream(), qq.data_ptr(), kc.data_ptr(), vc.data_ptr(), sl.data_ptr(), pt.data_ptr(),
-                                 B, Hq, Hkv, D, page, pt.shape[1], float(sm_scale), num_kv_splits, ws.data_ptr(),
-                                 out.data_ptr(), lse.data_ptr())
+    rc = L.lib().b200_gqa_decode_ex(_stream(), qq.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), bstride, pstride,
+                                    hstride, sl.data_ptr(), pt.data_ptr(), B, Hq, Hkv, D, page, pt.shape[1], float(sm_scale),
+                                    num_kv_splits, ws.data_ptr(), out.data_ptr(), lse.data_ptr())
     L.check(rc, "b200_gqa_decode")
     return out, lse
+
+
+def gqa_qknorm_rope_cache_write(qkv: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.Tensor,
+                                slot_mapping: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, num_heads: int,
+                                num_kv_heads: int, q_norm_weight: torch.Tensor | None = None,
+                                k_norm_weight: torch.Tensor | None = None, eps: float = 1e-6,
+                                is_neox_style: bool = True) -> torch.Tensor:
+    """One launch for the attention block's work before decode: per-head RMSNorm of q and k (Qwen3, reference
+    models/qwen3_moe.py:333-351; skipped where the weight is None), RoPE of q and k (fused_qk_norm_rope,
+    vllm/_custom_ops.py:279) and reshape_and_cache_flash of the new k / v (csrc/libtorch_stable/cache_kernels.cu:315-400).
+    qkv [T, (Hq + 2 Hkv) * 128] bf16 (the fused QKV projection's rows); positions [T] (clamped to the table's rows);
+    cos_sin_cache bf16 [max_position, rotary_dim] = cos | sin; slot_mapping [T] (< 0: padded token, nothing written);
+    k_cache / v_cache the views exactly as the reference passes them to reshape_and_cache_flash.
+    Returns q_out [T, Hq, 128] bf16, contiguous: the q that gqa_decode takes."""
+    x = _cuda(qkv, "qkv")
+    if x.dtype != torch.bfloat16 or x.dim() != 2 or x.shape[1] != (num_heads + 2 * num_kv_heads) * 128:
+        raise ValueError(f"qkv must be bf16 [T, (num_heads + 2 * num_kv_heads) * 128], got {x.dtype} {tuple(x.shape)}")
+    cs = _cuda(cos_sin_cache, "cos_sin_cache")
+    if cs.dtype != torch.bfloat16 or cs.dim() != 2:
+        raise ValueError("cos_sin_cache must be bf16 [max_position, rotary_dim]")
+    bstride, pstride, hstride = _kv_cache_strides(k_cache, v_cache)
+    if k_cache.shape[2] != num_kv_heads or k_cache.device != x.device:
+        raise ValueError("the cache views must hold num_kv_heads heads on qkv's device")
+    ws = []
+    for w, n in ((q_norm_weight, "q_norm_weight"), (k_norm_weight, "k_norm_weight")):
+        if w is not None:
+            w = _cuda(w, n)
+            if w.dtype != torch.bfloat16 or w.numel() != 128:
+                raise ValueError(f"{n} must be bf16 [128]")
+        ws.append(w)
+    T = x.shape[0]
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    sm = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
+    if pos.numel() != T or sm.numel() != T:
+        raise ValueError("positions and slot_mapping need one entry per token")
+    q_out = torch.empty(T, num_heads, 128, dtype=torch.bfloat16, device=x.device)
+    rc = L.lib().b200_gqa_qknorm_rope_cache_write(
+        _stream(), x.data_ptr(), pos.data_ptr(), cs.data_ptr(), cs.shape[0], cs.shape[1], int(is_neox_style),
+        ws[0].data_ptr() if ws[0] is not None else None, ws[1].data_ptr() if ws[1] is not None else None, float(eps),
+        sm.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), bstride, pstride, hstride, k_cache.shape[1],
+        q_out.data_ptr(), T, num_heads, num_kv_heads, 128)
+    L.check(rc, "b200_gqa_qknorm_rope_cache_write")
+    return q_out
