@@ -188,6 +188,14 @@ B200_DEVICE float fp8_group_scale(float absmax, int e8m0) {
   return sc;
 }
 
+// ----------------------------------------------------------------------------- register reallocation
+// Every warp of a warpgroup executes the same one.  `inc` blocks until other warpgroups have released enough registers
+// with `dec`: the sum over the CTA must stay within what the launch allocated (registers of the kernel x threads).
+template <int R>
+B200_DEVICE void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+B200_DEVICE void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // ----------------------------------------------------------------------------- misc
 B200_DEVICE float warp_max(float v) {
 #pragma unroll

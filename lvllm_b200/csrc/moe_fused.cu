@@ -19,6 +19,9 @@
 // are ONE copy each), MMA warpgroup (wgmma, register accumulators parked in the exchange area of common.cuh), 4 drain
 // warps (FP8 block-scale promotion, activation, stores).  The producer runs ahead across phase boundaries: weight tiles are
 // requested as soon as a ring slot frees up, the dependent B operand is requested when its flag is up.
+// 4-bit layers (W4A16) have two consumer warpgroups instead of the MMA warpgroup: each converts the raw nibbles of its
+// 64 weight rows straight from the stage into wgmma A fragments (registers) and multiplies them with the token tile
+// (shared memory); a chunk holds up to 64 rows of one expert, so a decode batch streams each active expert once.
 //
 // Roofline: HBM.  Algorithmic bytes per launch = weight bytes of the distinct active experts.
 #include <cstdio>
@@ -71,28 +74,34 @@ struct FusedArgs {
 };
 
 constexpr int W4_TILE_MAX = 4096 + 512;   // nibbles + scales of one [128 x 64] 4-bit tile
-constexpr int W4_NDQ = 2;                 // dequantised (fp16) A-operand ring depth (two 16 KB tiles per slot)
 
 template <bool FP8, int NA, int TNMAX, int WQ>
 struct FCfg {
-  // WQ: 0 none, 1 int4 / 2 nvfp4 / 3 mxfp4 dequantised to fp16 by CUDA cores (W4A16)
+  // WQ: 0 none, 1 int4 / 2 nvfp4 / 3 mxfp4 converted to fp16 wgmma A fragments in registers (W4A16)
   static constexpr int WD = WQ;
+  static constexpr int TN = TNMAX;
   // WD == 0: 32 KB of MMA-ready tiles per stage; WD != 0: two k-blocks x two raw 4-bit tiles per stage
   static constexpr int A_STAGE = WD ? 4 * W4_TILE_MAX : 2 * TILE_BYTES;
   static constexpr int B_STAGE = 2 * TNMAX * 128;   // up to two k-blocks of tn rows
   static constexpr int STAGE = A_STAGE + B_STAGE;
   static constexpr int TABLES = 24 * 1024;
-  static constexpr int DQ = WD ? W4_NDQ * 2 * TILE_BYTES : 0;   // ring of dequantised fp16 tile pairs (MMA-ready)
-  // warps 0-3 drain, 4 A-producer, 6-9 fix-up, 10 B-producer; WD: two dequant groups (warps 11-14, 15-18);
-  // last four warps: the MMA warpgroup
-  static constexpr int MMA_WARP0 = WQ ? 20 : 12;
-  static constexpr int NTHREADS = (MMA_WARP0 + 4) * 32;
+  // warps 0-3 drain, 4 A-producer, 6-9 fix-up, 10 B-producer; from warp 12: the MMA warpgroup (WD: two consumer
+  // warpgroups, rows [0,64) and [64,128) of the gate and up tiles)
+  static constexpr int MMA_WARP0 = 12;
+  static constexpr int MMA_THREADS = WD ? 256 : 128;
+  static constexpr int NTHREADS = MMA_WARP0 * 32 + MMA_THREADS;
+  // WD: registers after setmaxnreg (consumers / everything else); the pool is the launch's 65536 / NTHREADS rounded
+  // down to 8 per thread
+  static constexpr int REG_MMA = 120, REG_REST = 80;
+  static_assert(!WD || REG_MMA * MMA_THREADS + REG_REST * (NTHREADS - MMA_THREADS) <= (65536 / NTHREADS) / 8 * 8 * NTHREADS,
+                "register split exceeds the launch allocation");
   static constexpr int BUFCOLS = 2 * TNMAX;       // gate + up accumulators (GEMM2 uses the first TNMAX)
-  static constexpr int NBUF = 2;
+  // WD at 64 columns: one buffer (a tile accumulates over 32 stages, long enough for the drain to empty it)
+  static constexpr int NBUF = (WD && TNMAX == 64) ? 1 : 2;
   static constexpr int XCH = NBUF * BUFCOLS * 128 * 4;   // accumulator exchange area
-  static constexpr int STAGES_RAW = (F_SMEM_BUDGET - TABLES - DQ - XCH - 1024) / STAGE;
+  static constexpr int STAGES_RAW = (F_SMEM_BUDGET - TABLES - XCH - 1024) / STAGE;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-  static constexpr int SMEM = STAGES * STAGE + DQ + XCH + TABLES + 1024;
+  static constexpr int SMEM = STAGES * STAGE + XCH + TABLES + 1024;
   static_assert(STAGES >= 2, "shared-memory budget");
 };
 
@@ -107,7 +116,6 @@ struct __align__(16) FTables {
   uint64_t full[8], empty[8];
   uint64_t tfull[4], tempty[4];
   uint64_t qfull[F_QD], qempty[F_QD];
-  uint64_t dqfull[W4_NDQ], dqempty[W4_NDQ];
   int32_t n_chunks, n_rows, n_valid, flag;
   float red[F_EPI_WARPS][64];
   int16_t row_of_slot[FUSED_MAX_SLOTS];   // permuted row of slot, -1 = skipped
@@ -157,11 +165,6 @@ B200_DEVICE unsigned long long gtimer() {
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
   return t;
 }
-// cycle probes of the dequant role: compiled out unless -DF_PROBE=1
-#ifndef F_PROBE
-#define F_PROBE 0
-#endif
-#define F_CLK() (F_PROBE ? clock64() : 0ll)
 #define F_STAMP(idx)                                                   \
   do {                                                                 \
     if (a.dbg) a.dbg[(size_t)blockIdx.x * 16 + (idx)] = gtimer();      \
@@ -219,6 +222,192 @@ B200_DEVICE void combine_cols(const FusedArgs& a, const FTables* tb, int j, int 
   }
 }
 
+// ------------------------------------------------------------------------------- 4-bit consumer warpgroups
+// A raw [128 x 64] 4-bit tile stores each row's two 32-column halves as four words; word i holds columns 8i..8i+7 in the
+// order the conversion unpacks them (int4: nibbles j and j+4 -> columns 8i+2j, +1; e2m1: byte j -> columns 8i+2j, +1).
+// The wgmma A fragment of a k16 slice wants columns (2t, 2t+1) and (2t+8, 2t+9) of two rows (t = lane % 4): nibble pair /
+// byte t of the slice's two words.  The operation sequence per format is fixed, so the fp16 values are exactly those of
+// the dequantised tile: int4 (1024 + q) - 1032 then * scale; e2m1 bits placed at value * 2^-14, * 2^14, then * scale.
+template <int WQ>
+B200_DEVICE uint32_t w4_pair(uint32_t w, int t, __half2 s2) {
+  __half2 h;
+  if (WQ == 1) {
+    const uint32_t q = ((w >> (4 * t)) & 0x000F000Fu) | 0x64006400u;   // fp16 (1024 + q) pairs
+    h = __hmul2(__hadd2(*reinterpret_cast<const __half2*>(&q), __float2half2_rn(-1032.0f)), s2);   // q - 8 is exact
+  } else {
+    const uint32_t by = (w >> (8 * t)) & 0xFFu;
+    // sign to bit 15, exponent + mantissa to bits [11:9]: value * 2^-14 (the e2m1 subnormal 0.5 lands on an fp16 subnormal)
+    const uint32_t e = ((by & 0x7u) << 9) | ((by & 0x8u) << 12) | ((by & 0x70u) << 21) | ((by & 0x80u) << 24);
+    h = __hmul2(__hmul2(*reinterpret_cast<const __half2*>(&e), __float2half2_rn(16384.0f)), s2);
+  }
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+// scale of row r for the 16 columns [32 grp + 16 sub, +16)
+B200_DEVICE uint2 lds_u2(uint32_t addr) {
+  uint2 v;
+  asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
+  return v;
+}
+B200_DEVICE uint32_t lds_u16(uint32_t addr) {
+  uint16_t v;
+  asm volatile("ld.shared.b16 %0, [%1];" : "=h"(v) : "r"(addr));
+  return v;
+}
+B200_DEVICE uint32_t lds_u8(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+// scale of row r for the 16 columns [32 grp + 16 sub, +16) (sc: shared-memory address of the tile's scales)
+template <int WQ>
+B200_DEVICE __half2 w4_scale(uint32_t sc, int grp, int sub, int r) {
+  if (WQ == 1) {
+    const uint16_t b = (uint16_t)lds_u16(sc + (grp * 128 + r) * 2);
+    return __half2half2(*reinterpret_cast<const __half*>(&b));
+  }
+  if (WQ == 2) {
+    const __half_raw h = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)lds_u8(sc + (2 * grp + sub) * 128 + r), __NV_E4M3);
+    return __half2half2(*reinterpret_cast<const __half*>(&h));
+  }
+  // e8m0 -> fp16 2^(E-127): exponent field E-112 clamped to [0,30] (scales < 2^-14 flush to 0)
+  int f = (int)lds_u8(sc + grp * 128 + r) - 112;
+  f = f < 0 ? 0 : (f > 30 ? 30 : f);
+  const uint16_t bits = (uint16_t)(f << 10);
+  return __half2half2(*reinterpret_cast<const __half*>(&bits));
+}
+
+// k-iterations [ki0, ki1) of one tile at NN token columns: per k16 slice, convert the gate and up fragments of this
+// warpgroup's rows, then issue their two MMAs (A registers, B = token tile of the stage).  The conversion of a slice runs
+// while the MMAs of the previous one are in flight (wait_group 1); a stage is released once the MMAs of the next one
+// have been waited for, the last one of the tile after wait_group 0.
+// pins the accumulators in their registers across the asynchronous MMAs: without it the compiler may rematerialise or move
+// them, and ptxas then serialises every wgmma
+template <int N>
+B200_DEVICE void acc_fence(float (&acc)[2][N]) {
+#pragma unroll
+  for (int na = 0; na < 2; ++na)
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(acc[na][i])::"memory");
+}
+
+template <class C, int NN>
+B200_DEVICE void w4_tile(const FusedArgs& a, FTables* tb, const uint8_t* smem, int KB, int ki0, int ki1,
+                         float (&acc)[2][C::TN / 2], uint32_t& itc) {
+  constexpr int WQ = C::WD;
+  const int lane = threadIdx.x & 31;
+  const int r0 = (((int)threadIdx.x >> 7) - C::MMA_WARP0 / 4) * 64 + (((int)threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const int t = lane & 3;
+  const bool lead = (threadIdx.x & 127) == 0;
+  const uint32_t smem_u = smem_u32(smem);
+  int pend = -1;   // stage whose last MMAs may still be in flight
+  acc_fence(acc);
+  for (int ki = ki0; ki < ki1; ++ki, ++itc) {
+    const int s = itc % C::STAGES;
+    f_wait(&tb->full[s], (itc / C::STAGES) & 1);
+    const int kb0 = ki * 2;
+    const int nkb = (KB - kb0) < 2 ? (KB - kb0) : 2;
+    const uint32_t raw = smem_u + s * C::STAGE;
+    const uint32_t sb = raw + C::A_STAGE;
+    for (int kk = 0; kk < nkb; ++kk) {
+      const uint32_t bbase = sb + kk * (uint32_t)((NN >> 3) * 1024);
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const int grp = ks >> 1, sub = ks & 1;
+        uint32_t fa[2][4];
+#pragma unroll
+        for (int na = 0; na < 2; ++na) {
+          const uint32_t tile = raw + (kk * 2 + na) * a.w4_tile_bytes;
+          const uint2 q0 = lds_u2(tile + (grp * 128 + r0) * 16 + sub * 8);
+          const uint2 q1 = lds_u2(tile + (grp * 128 + r0 + 8) * 16 + sub * 8);
+          const __half2 s0 = w4_scale<WQ>(tile + 4096, grp, sub, r0), s1 = w4_scale<WQ>(tile + 4096, grp, sub, r0 + 8);
+          fa[na][0] = w4_pair<WQ>(q0.x, t, s0);
+          fa[na][1] = w4_pair<WQ>(q1.x, t, s1);
+          fa[na][2] = w4_pair<WQ>(q0.y, t, s0);
+          fa[na][3] = w4_pair<WQ>(q1.y, t, s1);
+        }
+        const uint64_t bd = wgmma_desc_sw128(bbase + ks * 32, 1024);
+        const uint32_t accum = (ki > ki0 || kk > 0 || ks > 0) ? 1u : 0u;
+        wgmma_fence();
+        WgmmaRS<NN, 0>::mma(acc[0], fa[0], bd, accum);
+        WgmmaRS<NN, 0>::mma(acc[1], fa[1], bd, accum);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (pend >= 0) {
+          if (lead) mbar_arrive(&tb->empty[pend]);
+          pend = -1;
+        }
+      }
+    }
+    pend = s;
+  }
+  wgmma_wait<0>();
+  acc_fence(acc);
+  if (lead && pend >= 0) mbar_arrive(&tb->empty[pend]);
+}
+
+// Consumer warpgroup of the 4-bit variants: walks the same schedule as the producers and the drain; every finished
+// accumulator (this warpgroup's 64 rows of gate and up) is parked in the exchange area.  The instruction width follows
+// the chunk's padded row count, so a 16-row chunk pays for 16 columns of tensor work.
+template <class C>
+B200_DEVICE void w4_consumer(const FusedArgs& a, FTables* tb, const uint8_t* smem, uint32_t xch, const SegList& sl) {
+  constexpr int TNMAX = C::TN;
+  const int half = ((int)threadIdx.x >> 7) - C::MMA_WARP0 / 4;
+  float acc[2][TNMAX / 2];
+#pragma unroll
+  for (int na = 0; na < 2; ++na)
+#pragma unroll
+    for (int i = 0; i < TNMAX / 2; ++i) acc[na][i] = 0.f;
+  uint32_t itc = 0, acc_it = 0;
+  for (int si = 0; si < sl.n; ++si) {
+    const Seg& sg = sl.s[si];
+    const int KI = sg.KI, sg_end = sg.end;
+    const int KB = sg.ph == 0 ? a.KB1 : a.KB2;
+    int it = sg.begin;
+    while (it < sg_end) {
+      const int tile = it / KI, k0 = it % KI;
+      const int k1 = (KI - k0 < sg_end - it) ? KI : k0 + (sg_end - it);
+      const int tn = ((int)tb->chunks[sg.c0 + tile / sg.J].nrows + 15) & ~15;
+      const uint32_t buf = acc_it % C::NBUF;
+      const uint32_t base = xch + buf * C::BUFCOLS;
+      switch (tn) {
+        case 16:
+          w4_tile<C, 16>(a, tb, smem, KB, k0, k1, acc, itc);
+          f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+          xch_store_frag<16>(base, half, acc[0]);
+          xch_store_frag<16>(base + TNMAX, half, acc[1]);
+          break;
+        case 32:
+          if constexpr (TNMAX >= 32) {
+            w4_tile<C, 32>(a, tb, smem, KB, k0, k1, acc, itc);
+            f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+            xch_store_frag<32>(base, half, acc[0]);
+            xch_store_frag<32>(base + TNMAX, half, acc[1]);
+          }
+          break;
+        case 48:
+          if constexpr (TNMAX >= 48) {
+            w4_tile<C, 48>(a, tb, smem, KB, k0, k1, acc, itc);
+            f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+            xch_store_frag<48>(base, half, acc[0]);
+            xch_store_frag<48>(base + TNMAX, half, acc[1]);
+          }
+          break;
+        default:
+          if constexpr (TNMAX >= 64) {
+            w4_tile<C, 64>(a, tb, smem, KB, k0, k1, acc, itc);
+            f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+            xch_store_frag<64>(base, half, acc[0]);
+            xch_store_frag<64>(base + TNMAX, half, acc[1]);
+          }
+          break;
+      }
+      mbar_arrive(&tb->tfull[buf]);
+      ++acc_it;
+      it += k1 - k0;
+    }
+  }
+}
+
 template <bool FP8, int NA, int TNMAX, int WQ>
 __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     moe_fused_kernel(const __grid_constant__ FusedArgs a) {
@@ -228,9 +417,9 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
   constexpr int WD = C::WD;     // dequant flavour
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* dq_ring = smem + C::STAGES * C::STAGE;
-  const uint32_t xch = xch_base(dq_ring + C::DQ);
-  FTables* tb = reinterpret_cast<FTables*>(dq_ring + C::DQ + C::XCH);
+  uint8_t* xch_area = smem + C::STAGES * C::STAGE;
+  const uint32_t xch = xch_base(xch_area);
+  FTables* tb = reinterpret_cast<FTables*>(xch_area + C::XCH);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int G = gridDim.x, cta = blockIdx.x;
@@ -240,19 +429,15 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     F_STAMP(0);
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&tb->full[i], 1);
-      mbar_init(&tb->empty[i], 1);
+      mbar_init(&tb->empty[i], C::MMA_THREADS / 128);   // one arrival per MMA warpgroup
     }
     for (int i = 0; i < C::NBUF; ++i) {
-      mbar_init(&tb->tfull[i], 128);   // every MMA thread, after parking its fragment
+      mbar_init(&tb->tfull[i], C::MMA_THREADS);   // every MMA thread, after parking its fragment
       mbar_init(&tb->tempty[i], F_EPI_WARPS);
     }
     for (int i = 0; i < F_QD; ++i) {
       mbar_init(&tb->qfull[i], F_EPI_WARPS);
       mbar_init(&tb->qempty[i], F_EPI_WARPS);
-    }
-    for (int i = 0; i < W4_NDQ; ++i) {
-      mbar_init(&tb->dqfull[i], 4);   // one elected arrival per dequant warp of the owning group
-      mbar_init(&tb->dqempty[i], 1);
     }
     fence_barrier_init();
   }
@@ -396,17 +581,17 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
   // are dealt round-robin to the CTAs; chunk-contiguous tiled layout:
   //   xt[row0_q * KB*128 + kb * (tn_q/8*1024) + ((r-row0_q)/8)*1024 + sw128((r-row0_q)%8, byte)]
   const int SEGS = (a.H + 1023) / 1024;
-  // gather groups of 128 threads: the drain warps, the fix-up warps and (4-bit formats) the dequant warps —
-  // none of them has anything else to do before the first accumulator is complete
-  const int ggrp = warp < 4 ? 0 : (warp >= 6 && warp < 10) ? 1 : (WQ && warp >= 11 && warp < 19) ? 2 + ((warp - 11) >> 2) : -1;
+  // gather groups of 128 threads: the drain warps, the fix-up warps and (4-bit formats) the consumer warpgroups —
+  // none of them has anything else to do before the first rows are gathered
+  const int ggrp = warp < 4 ? 0 : (warp >= 6 && warp < 10) ? 1 : (WQ && warp >= C::MMA_WARP0) ? 2 + ((warp - C::MMA_WARP0) >> 2) : -1;
   constexpr int NGG = WQ ? 4 : 2;
   if (ggrp >= 0) {
-    const int gt = ggrp == 0 ? tid : ggrp == 1 ? tid - 192 : tid - 352 - (ggrp - 2) * 128;   // 0..127
+    const int gt = ggrp == 0 ? tid : ggrp == 1 ? tid - 192 : tid - C::MMA_WARP0 * 32 - (ggrp - 2) * 128;   // 0..127
     int mine = 0;
     const int vcta = cta * NGG + ggrp, VG = G * NGG;
     // A round = GSL slots x all of their 1024-element segments (<= 8: H <= 8192): the routing metadata of a slot is
     // looked up once, and every 16-byte row load of the round is in flight before the first conversion starts
-    constexpr int GSL = WD ? 1 : 2;   // dequant variants: 104 registers per thread
+    constexpr int GSL = WD ? 1 : 2;   // 4-bit variants: 640 threads, 96 registers
     for (int sb = vcta; sb < n_slots; sb += GSL * VG) {
       uint4 raw[GSL][8];
       int rr_[GSL], row0_[GSL], tn_[GSL], r_[GSL];
@@ -570,6 +755,12 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     return;
   }
 
+  if constexpr (WD != 0) {
+    // the consumer warpgroups hold 2 x 32 fp32 accumulators per thread at 64 columns: registers move to them from the
+    // producer, drain and fix-up warps (the consumers take them in their own branch)
+    if (warp < C::MMA_WARP0) setmaxnreg_dec<C::REG_REST>();
+  }
+
   if (warp == 4 || warp == 10) {
     // ======================================================================= producers
     // warp 4 streams the weight stages (A), warp 10 the activation stages (B): two independent issue
@@ -655,7 +846,12 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
       }
       if (is_a) F_STAMP(6);
     }
-  } else if (warp >= C::MMA_WARP0) {
+  } else if (WD && warp >= C::MMA_WARP0) {
+    // ======================================================================= consumer warpgroups (4-bit formats)
+    setmaxnreg_inc<C::REG_MMA>();
+    w4_consumer<C>(a, tb, smem, xch, sl);
+    setmaxnreg_dec<C::REG_REST>();   // the combine below runs at the same count in every warp
+  } else if (!WD && warp >= C::MMA_WARP0) {
     // ======================================================================= MMA warpgroup
     // Walks the schedule with register accumulators: acc[na][h] = accumulator na (gate | up, or tile of a pair), rows
     // [64h, 64h + 64).  The instruction shape is fixed at N = TNMAX columns; columns beyond the chunk's rows multiply
@@ -663,11 +859,8 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     // the drain warps; the buffer is waited for only then, so its MMAs ran while the drain still read the previous one.
     const bool mma_lead = tid == C::MMA_WARP0 * 32;
     const uint32_t smem_base_u = smem_u32(smem);
-    const uint32_t dq_base_u = smem_u32(dq_ring);
     float acc[2][2][TNMAX / 2];
-    uint32_t itc = 0, acc_it = 0, dq_it = 0;
-    (void)dq_it;
-    (void)dq_base_u;
+    uint32_t itc = 0, acc_it = 0;
     for (int si = 0; si < sl.n; ++si) {
       const Seg& sg = sl.s[si];
       const int KI = sg.KI, sg_end = sg.end;
@@ -702,22 +895,7 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
           for (int kk = 0; kk < nkb; ++kk) {
             const uint32_t bbase = sb + kk * (uint32_t)((tn >> 3) * 1024);
             const uint32_t acc0 = (ki > k0 || kk > 0) ? 1u : 0u;
-            if (WD) {
-              // A operands come from the ring of dequantised fp16 tile pairs, B from the raw stage
-              const int d = dq_it % W4_NDQ;
-              f_wait(&tb->dqfull[d], (dq_it / W4_NDQ) & 1);
-              const uint32_t da = dq_base_u + d * 2 * TILE_BYTES;
-              wgmma_fence();
-#pragma unroll
-              for (int na = 0; na < 2; ++na)
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks)
-                  wgmma_tile128<TNMAX, 0>(acc[na], da + na * TILE_BYTES + ks * 32, bbase + ks * 32, ks > 0 ? 1u : acc0);
-              wgmma_commit();
-              wgmma_wait<0>();
-              if (mma_lead) mbar_arrive(&tb->dqempty[d]);
-              ++dq_it;
-            } else {
+            {
               const uint32_t a0 = sa + (two ? 0 : kk) * TILE_BYTES;
               wgmma_fence();
               if (a.dbg_mode != 2) {
@@ -932,114 +1110,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
       }
       if (tid == 0) F_STAMP(sg.ph == 0 ? 7 : 8);
     }
-  } else if (WD != 0 && warp >= 11) {
-    // ======================================================================= dequant warps 11..18 (4-bit formats)
-    // raw stage (two k-blocks x two [128 x 64] 4-bit tiles + scales) -> fp16 MMA operand tiles (128B swizzle)
-    // thread = tile row; per tile two 16-byte units (32 columns each) -> 4 x STS.128 each (conflict-free: the
-    // swizzle spreads 8 consecutive rows over the 8 chunk positions)
-    const int r = (warp & 3) * 32 + lane;   // tile row
-    const uint32_t grp = (uint32_t)(warp - 11) >> 2;   // two dequant groups alternate k-blocks
-    uint32_t cur = 0, dq_it = 0;
-    long long cyc_full = 0, cyc_slot = 0, cyc_math = 0, cyc_fence = 0, n_kb = 0;
-    for (int si = 0; si < sl.n; ++si) {
-      const Seg& sg = sl.s[si];
-      const int KB = sg.ph == 0 ? a.KB1 : a.KB2;
-      const int KI = sg.KI;
-      int ki = sg.begin % KI;
-      for (int it = sg.begin; it < sg.end; ++it, ++cur) {
-        const uint32_t s = cur % C::STAGES;
-        const long long c0 = F_CLK();
-        f_wait(&tb->full[s], (cur / C::STAGES) & 1);
-        cyc_full += F_CLK() - c0;
-        const int kb0 = ki * 2;
-        const int nkb = (KB - kb0) < 2 ? (KB - kb0) : 2;
-        const uint8_t* raw = smem + s * C::STAGE;
-        for (int kk = 0; kk < nkb; ++kk, ++dq_it) {
-          if ((dq_it & 1u) != grp) continue;
-          const int d = dq_it % W4_NDQ;
-          const long long c1 = F_CLK();
-          f_wait(&tb->dqempty[d], ((dq_it / W4_NDQ) & 1) ^ 1);
-          const long long c2 = F_CLK();
-          cyc_slot += c2 - c1;
-          uint8_t* dst = dq_ring + d * 2 * TILE_BYTES;
-#pragma unroll
-          for (int na = 0; na < 2; ++na) {
-            const uint8_t* tile = raw + (kk * 2 + na) * a.w4_tile_bytes;
-            const uint8_t* sc = tile + 4096;
-#pragma unroll
-            for (int g = 0; g < 2; ++g) {
-              const uint4 q = *reinterpret_cast<const uint4*>(tile + (g * 128 + r) * 16);
-              const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-              __half2 o[16];
-              if (WQ == 1) {
-                const __half sh = reinterpret_cast<const __half*>(sc)[g * 128 + r];
-                const __half2 s2 = __half2half2(sh);
-                const __half2 off = __float2half2_rn(-1032.0f);
-#pragma unroll
-                for (int wi = 0; wi < 4; ++wi) {
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    const uint32_t t = ((w[wi] >> (4 * j)) & 0x000F000Fu) | 0x64006400u;   // fp16 (1024 + q) pairs
-                    const __half2 hq = __hadd2(*reinterpret_cast<const __half2*>(&t), off);  // q - 8, exact
-                    o[wi * 4 + j] = __hmul2(hq, s2);
-                  }
-                }
-              } else {
-                __half2 s2[2];
-                if (WQ == 2) {
-                  const __half_raw h0 = __nv_cvt_fp8_to_halfraw(sc[(2 * g) * 128 + r], __NV_E4M3);
-                  const __half_raw h1 = __nv_cvt_fp8_to_halfraw(sc[(2 * g + 1) * 128 + r], __NV_E4M3);
-                  s2[0] = __half2half2(*reinterpret_cast<const __half*>(&h0));
-                  s2[1] = __half2half2(*reinterpret_cast<const __half*>(&h1));
-                } else {
-                  // e8m0 -> fp16 2^(E-127): exponent field E-112 clamped to [0,30] (scales < 2^-14 flush to 0)
-                  int f = (int)sc[g * 128 + r] - 112;
-                  f = f < 0 ? 0 : (f > 30 ? 30 : f);
-                  const uint16_t bits = (uint16_t)(f << 10);
-                  s2[0] = s2[1] = __half2half2(*reinterpret_cast<const __half*>(&bits));
-                }
-#pragma unroll
-                for (int wi = 0; wi < 4; ++wi) {
-                  // e2m1 nibble -> fp16: sign to bit 15, exponent + mantissa to bits [11:9] give value * 2^-14 (the
-                  // e2m1 subnormal 0.5 lands on an fp16 subnormal), so one exact multiplication by 2^14 finishes it
-                  uint32_t h[4];
-                  const __half2 k14 = __float2half2_rn(16384.0f);
-#pragma unroll
-                  for (int b = 0; b < 4; ++b) {
-                    const uint32_t by = (w[wi] >> (8 * b)) & 0xFFu;
-                    const uint32_t t = ((by & 0x7u) << 9) | ((by & 0x8u) << 12) | ((by & 0x70u) << 21) | ((by & 0x80u) << 24);
-                    const __half2 hv = __hmul2(*reinterpret_cast<const __half2*>(&t), k14);
-                    h[b] = *reinterpret_cast<const uint32_t*>(&hv);
-                  }
-#pragma unroll
-                  for (int b = 0; b < 4; ++b)
-                    o[wi * 4 + b] = __hmul2(*reinterpret_cast<const __half2*>(&h[b]), s2[wi >> 1]);
-                }
-              }
-              // 32 K values = 64 bytes = four 16-byte chunks of this row in the swizzled tile
-#pragma unroll
-              for (int i = 0; i < 4; ++i)
-                *reinterpret_cast<uint4*>(dst + na * TILE_BYTES + sw128_offset(r, g * 64 + i * 16)) = reinterpret_cast<const uint4*>(o)[i];
-            }
-          }
-          const long long c3 = F_CLK();
-          cyc_math += c3 - c2;
-          fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tb->dqfull[d]);
-          cyc_fence += F_CLK() - c3;
-          ++n_kb;
-        }
-        if (++ki == KI) ki = 0;
-      }
-    }
-    if (F_PROBE && a.dbg && a.dbg_mode != 5 && warp == 11 && lane == 0) {
-      unsigned long long* o = a.dbg + (size_t)blockIdx.x * 16 + 12;
-      o[0] = (unsigned long long)(n_kb ? cyc_full / n_kb : 0);
-      o[1] = (unsigned long long)(n_kb ? cyc_slot / n_kb : 0);
-      o[2] = (unsigned long long)(n_kb ? cyc_math / n_kb : 0);
-      o[3] = (unsigned long long)(n_kb ? cyc_fence / n_kb : 0);
-    }
   } else if (warp >= 6 && warp < 10) {
     // ======================================================================= fix-up warps 6..9
     // stream-K reduction, activation / requantisation / publication, combine: everything that has a
@@ -1091,10 +1161,10 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
           if (!WQ && ftid == 0 && a.dbg && ph == 0) a.dbg[(size_t)blockIdx.x * 16 + 12] = gtimer() - tA;
         }
         const unsigned long long tB = gtimer();
-        // Finalisation runs in blocks of FB token columns so that every array stays in registers: the 768-thread
-        // 4-bit variants have 85 registers per thread, and whole-tile arrays (acc[2][32] + tmp[4][32]) would live in
+        // Finalisation runs in blocks of FB token columns so that every array stays in registers: the fix-up warps of
+        // the 4-bit variants have 80 registers per thread, and whole-tile arrays (acc[2][32] + tmp[4][32]) would live in
         // local memory, serialising the L2 round trips.
-        constexpr int FB = WD ? 8 : 16;   // dequant variants: 768 threads, 85 registers
+        constexpr int FB = WD ? 8 : 16;
         if (finalize) {
           const float* own = a.partials + ((size_t)(4 * G * 2) + (size_t)cta * F_QD + qe) * (size_t)(2 * TNMAX * 128);
           // NVFP4 per-expert global scales (gate / up of w13, w2): linear, applied once to the reduced sums
@@ -1282,7 +1352,7 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
         else
           atomicAdd(&sy->comb[0], pend_n);
       }
-      if (WQ && !F_PROBE && ftid == 0 && a.dbg && si == sl.n - 1) a.dbg[(size_t)blockIdx.x * 16 + 12] = gtimer();   // fix-up role done
+      if (WQ && ftid == 0 && a.dbg && si == sl.n - 1) a.dbg[(size_t)blockIdx.x * 16 + 12] = gtimer();   // fix-up role done
 
     }
   }
@@ -1452,16 +1522,20 @@ int launch_fused(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const v
     a.align_g1 = g1 ? atoi(g1) : 60;   // percent of the CTA slots whole GEMM1 tiles must fill (0: always stream-K)
   }
   const bool fp8 = L->esz_bits == 8;
-  const int tn = M <= 16 ? 16 : 32;   // experts with more rows are processed in chunks of TNMAX
+  // experts with more rows are processed in chunks of TNMAX; 4-bit layers take chunks of up to 64 rows, so that at
+  // M <= 64 every active expert's weights are streamed once
+  const int tn = M <= 16 ? 16 : 32;
+  const int tn4 = M <= 16 ? 16 : M <= 32 ? 32 : 64;
 #define F_DISPATCH(FP8_, NA_)                                          \
   switch (tn) {                                                        \
     case 16: return launch_fused_t<FP8_, NA_, 16, 0>(a, st, num_sms);  \
     default: return launch_fused_t<FP8_, NA_, 32, 0>(a, st, num_sms);  \
   }
 #define F_DISPATCH_W4(WQ_)                                             \
-  switch (tn) {                                                        \
+  switch (tn4) {                                                       \
     case 16: return launch_fused_t<false, 2, 16, WQ_>(a, st, num_sms); \
-    default: return launch_fused_t<false, 2, 32, WQ_>(a, st, num_sms); \
+    case 32: return launch_fused_t<false, 2, 32, WQ_>(a, st, num_sms); \
+    default: return launch_fused_t<false, 2, 64, WQ_>(a, st, num_sms); \
   }
   if (L->wq == 1) { F_DISPATCH_W4(1) }
   if (L->wq == 2) { F_DISPATCH_W4(2) }
