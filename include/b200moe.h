@@ -177,7 +177,7 @@ int b200_rmsnorm_cast(void* stream, const float* in, void* out, int num_tokens, 
 /* ---- decode attention ----------------------------------------------------------------------------- */
 /* Paged MLA decode, absorbed form.  q_nope [B,Hq,512], q_pe [B,Hq,64] (bf16), kv cache
  * [num_pages,page_size,576] bf16, seq_lens int32 [B], page_table int32 [B,max_pages];
- * out bf16 [B,Hq,512], lse f32 [B,Hq] (may be NULL).  workspace: b200_mla_decode_workspace_bytes(). */
+ * out bf16 [B,Hq,512], lse f32 [B,Hq] (may be NULL); Hq <= 128.  workspace: b200_mla_decode_workspace_bytes(). */
 int64_t b200_mla_decode_workspace_bytes(int batch, int num_heads, int num_splits);
 int b200_mla_decode(void* stream, const void* q_nope, const void* q_pe, const void* kv_cache,
                     const int32_t* seq_lens, const int32_t* page_table, int batch, int num_heads,

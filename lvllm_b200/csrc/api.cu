@@ -47,10 +47,6 @@ static int check_device(int* dev_out) {
 // optional per-kernel timing of the two expert GEMMs (bench.py roofline): CUDA events recorded on the
 // launching stream around each GEMM when enabled and not capturing
 static bool g_profile = false;
-static bool g_use_fused = []() {
-  const char* v = getenv("B200MOE_DISABLE_FUSED");
-  return !(v && v[0] == '1');
-}();
 struct EvTriple { cudaEvent_t e[3];   bool fused = false;   // one kernel: only e[0]..e[1] is meaningful
 };
 static std::vector<EvTriple> g_events;
@@ -194,7 +190,7 @@ static int forward_device(b200moe_layer* L, cudaStream_t st, int M, int k, const
     if (rc) return rc;
     const size_t osz = (out_dtype == 2) ? 4 : 2;
     void* optr = reinterpret_cast<uint8_t*>(out) + (size_t)t0 * L->H * osz;
-    if (g_use_fused && fused_supported(L, m, k)) {
+    if (fused_supported(L, m, k)) {
       cudaEvent_t* fev = nullptr;
       if (g_profile && !cap) {
         fev = next_events(true);
@@ -677,7 +673,6 @@ int b200moe_debug_read(int what, void* dst_host, int64_t bytes) {
     case 6: src = ws->chunks; break;
     case 7: src = ws->row_of_slot; break;
     case 8: src = ws->slot_of_row; break;
-    case 9: src = ws->dbg; ws->dbg_enabled = true; break;   // also arms the stamps for later launches
     default: break;
   }
   if (!src || !dst_host || bytes <= 0) {

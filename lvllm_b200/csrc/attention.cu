@@ -1,20 +1,21 @@
-// Paged decode attention (one query token per request), split-KV + LSE merge.
+// Paged decode attention (one query token per request), split-KV + LSE merge: the entry points, the split merges and
+// the CUDA-core GQA kernel.
 //   MLA (absorbed): q = [q_nope(512) | q_pe(64)], one shared latent KV head, K = all 576 cols, V = first 512
-//                   (op contract of reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262)
+//                   (op contract of reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262);
+//                   up to 128 heads, on the tensor-core kernel (attention_mla.cu)
 //   GQA           : q [B,Hq,D], K / V caches [pages,page,Hkv,D] given by base pointer + (page, slot, head) strides:
 //                   separate contiguous caches or the halves of the FlashInfer backend's packed NHD / HND cache
-//                   (reference tests/kernels/attention/test_flashinfer.py:29-80)
+//                   (reference tests/kernels/attention/test_flashinfer.py:29-80); the tensor-core kernel
+//                   (attention_gqa.cu) where it applies, decode_attn_kernel otherwise
 //
-// v1 kernel (CUDA cores): a CTA owns (request, kv-head, head-group, split); KV tiles of TOK tokens are staged
+// decode_attn_kernel (CUDA cores): a CTA owns (request, kv-head, head-group, split); KV tiles of TOK tokens are staged
 // ONCE in shared memory with 16-byte coalesced loads and shared by all heads of the group (one warp per q
 // head), so HBM traffic == algorithmic KV bytes; the warp does the dot product over its lane-strided dims,
-// online softmax in fp32 (exp2 domain), and accumulates V.  Partial (o, m, l) per split are merged by
-// a second tiny kernel that also emits the natural-log LSE.
-// Roofline: HBM (KV bytes) for GQA at batch; latency/FMA bound for MLA at B=1 (tensor-core version is the
-// follow-up, see DESIGN.md).
+// online softmax in fp32 (exp2 domain), and accumulates V.  It serves groups of more than 32 query heads per kv head,
+// more work items per CTA than the tensor-core kernel's table holds, and split counts that do not cover the page table.
+// Partial (o, m, l) per split are merged by a second tiny kernel that also emits the natural-log LSE.
+// Roofline: HBM (KV bytes).
 #include <math_constants.h>
-
-#include <cstdlib>
 
 #include "common.cuh"
 #include "moe_internal.cuh"
@@ -23,16 +24,15 @@ namespace b200 {
 
 constexpr int ATT_TOK = 16;  // tokens per smem tile
 
-template <int DK, int DV, int WARPS, bool MLA>
+template <int DK, int DV, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
-    decode_attn_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ q2,
-                       const __nv_bfloat16* __restrict__ kc, const __nv_bfloat16* __restrict__ vc,
-                       const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ page_table, int Hq, int Hkv,
-                       int page_size, int max_pages, float scale_log2, int num_splits, float* __restrict__ part_o,
-                       float* __restrict__ part_ml, int64_t block_stride, int64_t page_stride, int64_t head_stride) {
+    decode_attn_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
+                       const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ seq_lens,
+                       const int32_t* __restrict__ page_table, int Hq, int Hkv, int page_size, int max_pages,
+                       float scale_log2, int num_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
+                       int64_t block_stride, int64_t page_stride, int64_t head_stride) {
   // blockIdx.x = ((b * Hkv + hkv) * groups_per_kv + hg), blockIdx.y = split
-  // GQA: K / V row of (page, slot in page, kv head) at page * block_stride + slot * page_stride + hkv * head_stride
-  // (elements); MLA: the latent cache is contiguous and the strides are unused
+  // K / V row of (page, slot in page, kv head) at page * block_stride + slot * page_stride + hkv * head_stride (elements)
   const int G = Hq / Hkv;
   const int groups_per_kv = (G + WARPS - 1) / WARPS;
   int bx = blockIdx.x;
@@ -52,22 +52,12 @@ __global__ void __launch_bounds__(WARPS * 32)
   const int s1 = min(S, s0 + per);
 
   __shared__ __align__(16) __nv_bfloat16 ks[ATT_TOK][DK];
-  __shared__ __align__(16) __nv_bfloat16 vs[MLA ? 1 : ATT_TOK][MLA ? 8 : DV];
+  __shared__ __align__(16) __nv_bfloat16 vs[ATT_TOK][DV];
 
   constexpr int NK = DK / 32, NV = DV / 32;
   float qr[NK];
 #pragma unroll
-  for (int i = 0; i < NK; ++i) {
-    const int d = lane + 32 * i;
-    float v;
-    if (MLA) {
-      v = (d < 512) ? __bfloat162float(q[((size_t)b * Hq + hq) * 512 + d])
-                    : __bfloat162float(q2[((size_t)b * Hq + hq) * 64 + (d - 512)]);
-    } else {
-      v = __bfloat162float(q[((size_t)b * Hq + hq) * DK + d]);
-    }
-    qr[i] = v * scale_log2;
-  }
+  for (int i = 0; i < NK; ++i) qr[i] = __bfloat162float(q[((size_t)b * Hq + hq) * DK + lane + 32 * i]) * scale_log2;
   float o[NV];
 #pragma unroll
   for (int i = 0; i < NV; ++i) o[i] = 0.f;
@@ -76,29 +66,25 @@ __global__ void __launch_bounds__(WARPS * 32)
   for (int t0 = s0; t0 < s1; t0 += ATT_TOK) {
     const int nt = min(ATT_TOK, s1 - t0);
     __syncthreads();
-    // cooperative 16-byte loads of the K (and V) rows of this tile
+    // cooperative 16-byte loads of the K and V rows of this tile
     constexpr int KCH = DK / 8;
     for (int i = threadIdx.x; i < ATT_TOK * KCH; i += WARPS * 32) {
       const int tt = i / KCH, c = i % KCH;
       if (tt < nt) {
         const int tok = t0 + tt;
         const int page = page_table[(size_t)b * max_pages + tok / page_size];
-        const size_t row = (size_t)page * page_size + tok % page_size;
-        const __nv_bfloat16* src =
-            MLA ? kc + row * DK : kc + page * block_stride + (tok % page_size) * page_stride + hkv * head_stride;
+        const __nv_bfloat16* src = kc + page * block_stride + (tok % page_size) * page_stride + hkv * head_stride;
         *reinterpret_cast<uint4*>(&ks[tt][c * 8]) = *reinterpret_cast<const uint4*>(src + c * 8);
       }
     }
-    if (!MLA) {
-      constexpr int VCH = DV / 8;
-      for (int i = threadIdx.x; i < ATT_TOK * VCH; i += WARPS * 32) {
-        const int tt = i / VCH, c = i % VCH;
-        if (tt < nt) {
-          const int tok = t0 + tt;
-          const int page = page_table[(size_t)b * max_pages + tok / page_size];
-          *reinterpret_cast<uint4*>(&vs[MLA ? 0 : tt][c * 8]) = *reinterpret_cast<const uint4*>(
-              vc + page * block_stride + (tok % page_size) * page_stride + hkv * head_stride + c * 8);
-        }
+    constexpr int VCH = DV / 8;
+    for (int i = threadIdx.x; i < ATT_TOK * VCH; i += WARPS * 32) {
+      const int tt = i / VCH, c = i % VCH;
+      if (tt < nt) {
+        const int tok = t0 + tt;
+        const int page = page_table[(size_t)b * max_pages + tok / page_size];
+        *reinterpret_cast<uint4*>(&vs[tt][c * 8]) = *reinterpret_cast<const uint4*>(
+            vc + page * block_stride + (tok % page_size) * page_stride + hkv * head_stride + c * 8);
       }
     }
     __syncthreads();
@@ -128,10 +114,7 @@ __global__ void __launch_bounds__(WARPS * 32)
         const float p = (tt < nt) ? exp2f(sc[tt] - mt) : 0.f;
         l += p;
 #pragma unroll
-        for (int i = 0; i < NV; ++i) {
-          const float v = MLA ? __bfloat162float(ks[tt][lane + 32 * i]) : __bfloat162float(vs[MLA ? 0 : tt][(lane + 32 * i) % (MLA ? 8 : DV)]);
-          o[i] = fmaf(p, v, o[i]);
-        }
+        for (int i = 0; i < NV; ++i) o[i] = fmaf(p, __bfloat162float(vs[tt][lane + 32 * i]), o[i]);
       }
       m = mt;
     }
@@ -255,49 +238,26 @@ int b200_mla_decode_ex(void* stream, const void* q_nope, const void* q_pe, int q
                        const int32_t* page_table, int batch, int num_heads, int page_size, int max_pages, float sm_scale,
                        int num_splits, void* workspace, void* out, float* lse) {
   if (!q_nope || !q_pe || !kv_cache || !seq_lens || !page_table || !workspace || !out || batch <= 0 ||
-      num_heads <= 0 || page_size <= 0 || num_splits <= 0 || q_dtype < 0 || q_dtype > 1 || kv_dtype < 0 || kv_dtype > 1) {
-    set_error("b200_mla_decode: bad argument");
+      num_heads <= 0 || num_heads > 128 || page_size <= 0 || num_splits <= 0 || q_dtype < 0 || q_dtype > 1 ||
+      kv_dtype < 0 || kv_dtype > 1) {
+    set_error("b200_mla_decode: bad argument (num_heads <= 128)");
     return B200_ERR_INVALID;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  constexpr int WARPS = 8;
   float* po = reinterpret_cast<float*>(workspace);
   float* pml = po + (size_t)batch * num_heads * num_splits * 512;
-  // tensor-core path: one CTA per (request, 128-token split, value-dim half); needs the split count to cover
-  // the longest sequence the page table can describe (seq_lens live on the device)
-  static const bool use_tc = []() {
-    const char* v = getenv("B200_MLA_DISABLE_TC");
-    return !(v && v[0] == '1');
-  }();
-  if (use_tc && num_heads <= 128) {   // each CTA walks ceil(tiles / num_splits) 128-token tiles (online softmax)
-    int rc = launch_mla_tc(st, q_nope, q_pe, kv_cache, seq_lens, page_table, batch, num_heads, page_size, max_pages,
-                           sm_scale, num_splits, po, pml, kv_dtype, q_dtype, descale_q, descale_k);
-    if (rc) return rc;
-    if (num_splits <= 512)
-      mla_merge_kernel<<<batch * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
-    else
-      decode_merge_kernel<512><<<(batch * num_heads + 3) / 4, 128, 0, st>>>(po, pml, batch * num_heads, num_splits,
-                                                                           reinterpret_cast<__nv_bfloat16*>(out), lse);
-    ++g_launches;
-    cudaError_t e2 = cudaGetLastError();
-    if (e2 != cudaSuccess) return cuda_fail(e2, "mla merge launch");
-    return 0;
-  }
-  if (kv_dtype || q_dtype) {
-    set_error("b200_mla_decode: the e4m3 cache is served by the tensor-core kernel only (num_heads <= 128)");
-    return B200_ERR_INVALID;
-  }
-  const int groups = (num_heads + WARPS - 1) / WARPS;
-  dim3 grid(batch * groups, num_splits);
-  decode_attn_kernel<576, 512, WARPS, true><<<grid, WARPS * 32, 0, st>>>(
-      reinterpret_cast<const __nv_bfloat16*>(q_nope), reinterpret_cast<const __nv_bfloat16*>(q_pe),
-      reinterpret_cast<const __nv_bfloat16*>(kv_cache), nullptr, seq_lens, page_table, num_heads, 1, page_size,
-      max_pages, sm_scale * 1.4426950408889634f, num_splits, po, pml, 0, 0, 0);
-  decode_merge_kernel<512><<<(batch * num_heads + 3) / 4, 128, 0, st>>>(po, pml, batch * num_heads, num_splits,
-                                                                       reinterpret_cast<__nv_bfloat16*>(out), lse);
-  g_launches += 2;
+  // each CTA walks ceil(tiles / num_splits) 128-token tiles (online softmax)
+  int rc = launch_mla_tc(st, q_nope, q_pe, kv_cache, seq_lens, page_table, batch, num_heads, page_size, max_pages,
+                         sm_scale, num_splits, po, pml, kv_dtype, q_dtype, descale_q, descale_k);
+  if (rc) return rc;
+  if (num_splits <= 512)
+    mla_merge_kernel<<<batch * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
+  else
+    decode_merge_kernel<512><<<(batch * num_heads + 3) / 4, 128, 0, st>>>(po, pml, batch * num_heads, num_splits,
+                                                                         reinterpret_cast<__nv_bfloat16*>(out), lse);
+  ++g_launches;
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "mla_decode launch");
+  if (e != cudaSuccess) return cuda_fail(e, "mla merge launch");
   return 0;
 }
 
@@ -336,11 +296,7 @@ int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const v
   const float sl2 = sm_scale * 1.4426950408889634f;
   // tensor-core path (persistent CTAs over (request, kv head, 128-token split) items): needs the split count
   // to cover the longest sequence the page table can describe
-  static const bool use_tc = []() {
-    const char* v = getenv("B200_GQA_DISABLE_TC");
-    return !(v && v[0] == '1');
-  }();
-  if (use_tc && G <= 128 && num_splits <= 1024 && (int64_t)num_splits * 128 >= (int64_t)max_pages * page_size) {
+  if (G <= 128 && num_splits <= 1024 && (int64_t)num_splits * 128 >= (int64_t)max_pages * page_size) {
     const int rc = launch_gqa_tc(st, q, k_cache, v_cache, block_stride, page_stride, head_stride, seq_lens, page_table, batch,
                                  num_q_heads, num_kv_heads, page_size, max_pages, sm_scale, num_splits, po, pml, out, lse);
     if (rc <= 0) return rc;   // rc == 1: more work items per CTA than the kernel's table holds
@@ -349,8 +305,8 @@ int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const v
   {                                                                                                            \
     const int groups = (G + W - 1) / W;                                                                        \
     dim3 grid(batch * num_kv_heads * groups, num_splits);                                                      \
-    decode_attn_kernel<128, 128, W, false><<<grid, W * 32, 0, st>>>(                                           \
-        reinterpret_cast<const __nv_bfloat16*>(q), nullptr, reinterpret_cast<const __nv_bfloat16*>(k_cache),   \
+    decode_attn_kernel<128, 128, W><<<grid, W * 32, 0, st>>>(                                                  \
+        reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k_cache),            \
         reinterpret_cast<const __nv_bfloat16*>(v_cache), seq_lens, page_table, num_q_heads, num_kv_heads,      \
         page_size, max_pages, sl2, num_splits, po, pml, block_stride, page_stride, head_stride);               \
   }

@@ -41,9 +41,7 @@ struct GqaBars {
 
 // intra-CTA mbarrier wait (producer / MMA / softmax warps of ONE CTA: no other CTA or GPU is waited for).  A protocol bug
 // must not hang the box: back off after a while, trap after seconds.
-B200_DEVICE void gqa_wait(uint64_t* bar, uint32_t parity, int tag = 0, uint32_t n = 0) {
-  (void)tag;
-  (void)n;
+B200_DEVICE void gqa_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > (1u << 20)) __nanosleep(128);
@@ -134,7 +132,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
         uint8_t* q_t = stages + (size_t)s * stage_bytes;
         uint8_t* k_t = q_t + 2 * qbytes;
         uint8_t* v_t = k_t + 2 * TILE_BYTES;
-        gqa_wait(&bars->kv_free[s], ((n / NST) & 1) ^ 1, 1, n);
+        gqa_wait(&bars->kv_free[s], ((n / NST) & 1) ^ 1);
         for (int r = r0; r < N; r += 16) {
           const bool qok = r < G;
           const __nv_bfloat16* src = q + ((size_t)b * Hq + kvh * G + (qok ? r : 0)) * 128 + c * 8;
@@ -176,7 +174,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
     const uint32_t oa = smem_u32(ones);
     auto issue_qk = [&](uint32_t n) {
       const int s = n % NST, g = n & 1;
-      gqa_wait(&bars->qk_full[s], (n / NST) & 1, 2, n);
+      gqa_wait(&bars->qk_full[s], (n / NST) & 1);
       fence_proxy_async();   // LDGSTS (generic proxy) writes -> wgmma (async proxy) reads
       const uint32_t qa = smem_u32(stages + (size_t)s * stage_bytes), ka = qa + 2 * qbytes;
       float sacc[2][N / 2];                                               // A = K (K-major), B = Q (K-major)
@@ -190,15 +188,15 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       wgmma_wait<0>();
       // the columns still hold O^T of the group's previous item until its epilogue has read them (its PV was issued
       // before this QK, so the wait cannot block the MMAs it depends on)
-      if (n >= 2) gqa_wait(&bars->o_done[g], ((n >> 1) - 1) & 1, 7, n);
+      if (n >= 2) gqa_wait(&bars->o_done[g], ((n >> 1) - 1) & 1);
       xch_store_frag<N>(tm + g * N, 0, sacc[0]);
       xch_store_frag<N>(tm + g * N, 1, sacc[1]);
       mbar_arrive(&bars->s_full[g]);
     };
     auto issue_pv = [&](uint32_t n) {
       const int s = n % NST, g = n & 1;
-      gqa_wait(&bars->p_full[g], (n >> 1) & 1, 3, n);
-      gqa_wait(&bars->v_full[s], (n / NST) & 1, 4, n);
+      gqa_wait(&bars->p_full[g], (n >> 1) & 1);
+      gqa_wait(&bars->v_full[s], (n / NST) & 1);
       fence_proxy_async();
       const uint32_t va = smem_u32(stages + (size_t)s * stage_bytes) + 2 * qbytes + 2 * TILE_BYTES;
       const uint32_t pa = smem_u32(p_base + g * pbytes);
@@ -263,7 +261,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       }
       const uint32_t ph = (n >> 1) & 1;
       const bool tv = t < nt;
-      gqa_wait(&bars->s_full[g], ph, 5, n);
+      gqa_wait(&bars->s_full[g], ph);
       float my_ms = 0.f;                          // thread t == h keeps m[h] * scale for the partial record
       for (int c0 = 0; c0 < N; c0 += 16) {
         float v[16];
@@ -301,7 +299,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       }
       fence_proxy_async();
       mbar_arrive(&bars->p_full[g]);
-      gqa_wait(&bars->o_full[g], ph, 6, n);
+      gqa_wait(&bars->o_full[g], ph);
       // epilogue: thread = value dim d, columns = heads
       float* po = part_o + pbase * 128 + t;
       const size_t hstride = (size_t)num_splits * 128;

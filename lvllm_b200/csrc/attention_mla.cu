@@ -12,7 +12,7 @@
 // each: a thread keeps its share of S (64 fp32) and of O (64 fp32) in registers, the softmax runs on the accumulator
 // fragment (row statistics over the four threads of a quad) and P feeds the PV MMA as a register operand, so neither S
 // nor P touches shared memory.  A quarter of the value dims per CTA is what keeps both accumulators in registers.
-// Partial (O, m, l) per split are merged by decode_merge_kernel (attention.cu).
+// Partial (O, m, l) per split are merged by mla_merge_kernel (attention.cu), by decode_merge_kernel above 512 splits.
 //
 // Warp roles (384 threads): warps 0-3 / 4-7 consumer warpgroups (MMA + softmax + epilogue), warps 8-11 loaders
 // (16-byte gathers of q rows / paged KV rows -> swizzled smem, generic->async proxy fence).

@@ -68,8 +68,6 @@ struct FusedArgs {
   float* partials;
   FusedSync* sync;
   int rows_stride;
-  unsigned long long* dbg;  // optional [SMs][16] globaltimer stamps (bring-up / profiling aid)
-  int dbg_mode;             // bring-up only: 1 drain skips the accumulator loads + math, 2 the MMAs are skipped
   int align_g1;             // cut GEMM1 at tile boundaries too when whole tiles fill this percentage of <= 3 waves (B200MOE_ALIGN_G1, default 60)
 };
 
@@ -159,16 +157,6 @@ B200_DEVICE void finish_launch(FusedSync* sy, int n_chunks, int J2) {
   for (int i = 0; i < J2; ++i) sy->comb[i] = 0;
   __threadfence();
 }
-
-B200_DEVICE unsigned long long gtimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-#define F_STAMP(idx)                                                   \
-  do {                                                                 \
-    if (a.dbg) a.dbg[(size_t)blockIdx.x * 16 + (idx)] = gtimer();      \
-  } while (0)
 
 B200_DEVICE float f_silu(float x) { return x / (1.0f + expf(-x)); }
 B200_DEVICE float round_act(float v, int fp16) {
@@ -426,7 +414,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
   FusedSync* sy = a.sync;
 
   if (tid == 0) {
-    F_STAMP(0);
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&tb->full[i], 1);
       mbar_init(&tb->empty[i], C::MMA_THREADS / 128);   // one arrival per MMA warpgroup
@@ -539,7 +526,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     }
   }
   __syncthreads();
-  const int n_rows = tb->n_rows;
   const int n_chunks = tb->n_chunks;
   int n_valid_local = 0;
   for (int sidx = tid; sidx < n_slots; sidx += NT) {
@@ -575,7 +561,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     return;
   }
 
-  if (tid == 0) F_STAMP(1);
   // ------------------------------------------------------------------------------- phase 0b: row gather (+quant)
   // done by the four epilogue warps (the producer / MMA warps start streaming weights meanwhile); valid rows
   // are dealt round-robin to the CTAs; chunk-contiguous tiled layout:
@@ -690,7 +675,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
         atomicAdd(&sy->x_ready, mine);
       }
     }
-    if (tid == 0) F_STAMP(2);
   }
 
   // ------------------------------------------------------------------------------- stream-K schedule
@@ -743,18 +727,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     sl.n = n;
   }
 
-  if (a.dbg_mode == 3) {   // bring-up: print the schedule of the first CTAs and leave
-    if (tid == 0 && cta < 4) {
-      printf("cta %d: n_chunks %d n_rows %d n_valid %d NG %d KI1e %d KI2 %d J1 %d J2e %d KB1 %d KB2 %d tile_bytes %d\n", cta,
-             n_chunks, n_rows, n_valid, NG, KI1e, KI2, a.J1, J2e, a.KB1, a.KB2, a.w4_tile_bytes);
-      for (int i = 0; i < sl.n; ++i)
-        printf("   seg %d: ph %d c0 %d c1 %d KI %d J %d N %d P %d range [%d,%d)\n", i, sl.s[i].ph, sl.s[i].c0, sl.s[i].c1,
-               sl.s[i].KI, sl.s[i].J, sl.s[i].N, sl.s[i].P, sl.s[i].begin, sl.s[i].end);
-    }
-    __syncthreads();
-    return;
-  }
-
   if constexpr (WD != 0) {
     // the consumer warpgroups hold 2 x 32 fp32 accumulators per thread at 64 columns: registers move to them from the
     // producer, drain and fix-up warps (the consumers take them in their own branch)
@@ -771,7 +743,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
       const uint64_t pol = policy_evict_first();
       bool x_ok = false;
       int g1_ok_chunk = -1;
-      bool stamped5 = false;
       uint32_t cur = 0;  // flat iteration counter -> stage / parity
       for (int si = 0; si < sl.n; ++si) {
         const Seg& sg = sl.s[si];
@@ -813,16 +784,11 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
                 cnt_wait(&sy->x_ready, n_valid * SEGS);
                 asm volatile("fence.proxy.async.global;" ::: "memory");
                 x_ok = true;
-                F_STAMP(3);
               }
             } else if (g1_ok_chunk != q) {
               cnt_wait(&sy->g1_done[q], a.J1);
               asm volatile("fence.proxy.async.global;" ::: "memory");
               g1_ok_chunk = q;
-              if (!stamped5) {
-                F_STAMP(5);
-                stamped5 = true;
-              }
             }
             const uint8_t* base = ph1 ? a.xt : a.it;
             const uint8_t* bsrc = base + (size_t)ch.row0 * KB * 128 + (size_t)kb0 * ((tn >> 3) * 1024);
@@ -842,9 +808,7 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
             }
           }
         }
-        if (is_a && si == sl.n / 2 - 1) F_STAMP(4);
       }
-      if (is_a) F_STAMP(6);
     }
   } else if (WD && warp >= C::MMA_WARP0) {
     // ======================================================================= consumer warpgroups (4-bit formats)
@@ -898,20 +862,18 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
             {
               const uint32_t a0 = sa + (two ? 0 : kk) * TILE_BYTES;
               wgmma_fence();
-              if (a.dbg_mode != 2) {
 #pragma unroll
-                for (int na = 0; na < 2; ++na) {
-                  if (na < nacc) {
+              for (int na = 0; na < 2; ++na) {
+                if (na < nacc) {
 #pragma unroll
-                    for (int ks = 0; ks < 4; ++ks) {
-                      const uint32_t aa = a0 + na * TILE_BYTES + ks * 32, bb = bbase + ks * 32;
-                      if (FP8)
-                        wgmma_tile128<TNMAX, 2>(acc[na], aa, bb, ks > 0 ? 1u : 0u);
-                      else if (a.cmp_fp16)
-                        wgmma_tile128<TNMAX, 0>(acc[na], aa, bb, ks > 0 ? 1u : acc0);
-                      else
-                        wgmma_tile128<TNMAX, 1>(acc[na], aa, bb, ks > 0 ? 1u : acc0);
-                    }
+                  for (int ks = 0; ks < 4; ++ks) {
+                    const uint32_t aa = a0 + na * TILE_BYTES + ks * 32, bb = bbase + ks * 32;
+                    if (FP8)
+                      wgmma_tile128<TNMAX, 2>(acc[na], aa, bb, ks > 0 ? 1u : 0u);
+                    else if (a.cmp_fp16)
+                      wgmma_tile128<TNMAX, 0>(acc[na], aa, bb, ks > 0 ? 1u : acc0);
+                    else
+                      wgmma_tile128<TNMAX, 1>(acc[na], aa, bb, ks > 0 ? 1u : acc0);
                   }
                 }
               }
@@ -995,7 +957,7 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
             for (int w = 0; w < (TNMAX + 31) / 32; ++w) xs_cur[w] = tb->sc_x[rel][lane];
 #pragma unroll
             for (int na = 0; na < 2; ++na) {
-              if (na < nacc && a.dbg_mode != 1) {
+              if (na < nacc) {
 #pragma unroll
                 for (int c16 = 0; c16 < TNMAX / 16; ++c16) {
                   if (c16 * 16 < tn) {
@@ -1108,7 +1070,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
         }
         pend_y = 0;
       }
-      if (tid == 0) F_STAMP(sg.ph == 0 ? 7 : 8);
     }
   } else if (warp >= 6 && warp < 10) {
     // ======================================================================= fix-up warps 6..9
@@ -1147,7 +1108,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
           cf = part_owner(t_begin, sg.N, sg.P);
           cl = part_owner(t_last, sg.N, sg.P);
           int32_t* cnt = (ph == 0 ? sy->tcnt1 : sy->tcnt2) + (q * J + j);
-          const unsigned long long tA = gtimer();
           if (ftid == 0) {
             const int old = cnt_inc(cnt);
             if (old == cl - cf) *cnt = 0;   // last contributor: hand the counter back clean
@@ -1158,9 +1118,7 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
           asm volatile("bar.sync 2, 128;" ::: "memory");
           finalize = (arrived == cl - cf);
           if (finalize) __threadfence();  // acquire side of the contributor counter
-          if (!WQ && ftid == 0 && a.dbg && ph == 0) a.dbg[(size_t)blockIdx.x * 16 + 12] = gtimer() - tA;
         }
-        const unsigned long long tB = gtimer();
         // Finalisation runs in blocks of FB token columns so that every array stays in registers: the fix-up warps of
         // the 4-bit variants have 80 registers per thread, and whole-tile arrays (acc[2][32] + tmp[4][32]) would live in
         // local memory, serialising the L2 round trips.
@@ -1321,7 +1279,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
         __syncwarp();
         if (lane == 0) mbar_arrive(&tb->qempty[qe]);
         ++part_no;
-        if (!WQ && ftid == 0 && a.dbg && ph == 0 && finalize) a.dbg[(size_t)blockIdx.x * 16 + 13] = gtimer() - tB;
         if (finalize) {
           if (ph == 0) {
             // the intermediate is consumed through the async proxy (bulk copy) by other CTAs; publication of
@@ -1352,11 +1309,8 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
         else
           atomicAdd(&sy->comb[0], pend_n);
       }
-      if (WQ && ftid == 0 && a.dbg && si == sl.n - 1) a.dbg[(size_t)blockIdx.x * 16 + 12] = gtimer();   // fix-up role done
-
     }
   }
-  if (tid == 0) F_STAMP(9);
 
   // ---------------------------------------------------------------- phase 3: distributed combine (whole CTA)
   // out[t] = sum_j w[t,j] * y[row(t,j)] once every GEMM2 tile of the launch is finalised; every thread of every
@@ -1365,7 +1319,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
     if (tid == 0) cnt_wait(&sy->comb[0], n_chunks * J2e);
     __syncthreads();
     __threadfence();
-    if (tid == 0) F_STAMP(11);
     const int H4 = a.H >> 2, k = a.top_k;
     const int units = a.M * H4;
     for (int u = cta * NT + tid; u < units; u += G * NT) {
@@ -1407,7 +1360,6 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
         *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(a.out) + o) = pk;
       }
     }
-    if (tid == 0) F_STAMP(10);
   }
 
   __syncthreads();
@@ -1429,11 +1381,7 @@ static int launch_fused_t(const FusedArgs& a, cudaStream_t st, int num_sms) {
     attr_set = true;
   }
   // Cooperative launch: the cross-CTA spin waits need every CTA of the grid resident at once; a plain launch that
-  // shares the GPU with another stream's kernels could be scheduled piecemeal and dead-lock (B200MOE_COOP=0 reverts).
-  static const bool coop = []() {
-    const char* v = getenv("B200MOE_COOP");
-    return !(v && v[0] == '0');
-  }();
+  // shares the GPU with another stream's kernels could be scheduled piecemeal and dead-lock.
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(num_sms);
   cfg.blockDim = dim3(C::NTHREADS);
@@ -1443,7 +1391,7 @@ static int launch_fused_t(const FusedArgs& a, cudaStream_t st, int num_sms) {
   attr[0].id = cudaLaunchAttributeCooperative;
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = coop ? 1 : 0;
+  cfg.numAttrs = 1;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, a);
   ++g_launches;
   if (e != cudaSuccess) return cuda_fail(e, "moe_fused launch");
@@ -1514,13 +1462,8 @@ int launch_fused(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const v
   a.partials = ws->partials;
   a.sync = ws->fsync;
   a.rows_stride = (int)ws->cap_rows;
-  a.dbg = ws->dbg_enabled ? ws->dbg : nullptr;
-  {
-    const char* m = getenv("B200MOE_DBG_MODE");
-    a.dbg_mode = m ? atoi(m) : 0;
-    const char* g1 = getenv("B200MOE_ALIGN_G1");
-    a.align_g1 = g1 ? atoi(g1) : 60;   // percent of the CTA slots whole GEMM1 tiles must fill (0: always stream-K)
-  }
+  const char* g1 = getenv("B200MOE_ALIGN_G1");
+  a.align_g1 = g1 ? atoi(g1) : 60;   // percent of the CTA slots whole GEMM1 tiles must fill (0: always stream-K)
   const bool fp8 = L->esz_bits == 8;
   // experts with more rows are processed in chunks of TNMAX; 4-bit layers take chunks of up to 64 rows, so that at
   // M <= 64 every active expert's weights are streamed once

@@ -68,8 +68,6 @@ struct Workspace {  // process-wide, per device; sized for the largest layer / b
   float* y = nullptr;      // expert outputs fp32 [rows][H]
   float* partials = nullptr;   // stream-K partial tiles [2 phases][SMs][2][2*64*128] fp32
   FusedSync* fsync = nullptr;
-  unsigned long long* dbg = nullptr;   // [160][16] globaltimer stamps of the last fused launch
-  bool dbg_enabled = false;
   // host<->device staging of cpu_prefill
   void* d_hidden = nullptr;
   int32_t* d_ids = nullptr;

@@ -436,96 +436,6 @@ __global__ void __launch_bounds__(256) combine_kernel(const float* __restrict__ 
   }
 }
 
-// Second form of the combine (B200MOE_COMBINE=2): the token's VALID (row, weight) pairs are compacted first (j order kept),
-// and a thread holds all of its output positions (HV float4 columns, 1024 floats apart: H <= 8192 in one sweep) in
-// registers, so that every routed expert of the token costs ONE round of HV independent row loads.  On an EP shard most of
-// a token's k slots are not local (ids < 0): combine_kernel then has one live load per thread and sweep (the other seven of
-// its eight-wide round are predicated off).  Same fused multiply-adds in the same j order per output
-// element (skipped pairs contributed fma(0, 0, acc) = acc): bit-identical to combine_kernel.
-template <int HV>
-__global__ void __launch_bounds__(256) combine_v2_kernel(const float* __restrict__ y, const float* __restrict__ topk_w,
-                                                        const int32_t* __restrict__ row_of_slot, int top_k, int H,
-                                                        void* __restrict__ out, int out_dtype) {
-  __shared__ int s_row[64];
-  __shared__ float s_w[64];
-  __shared__ int s_n;
-  const int t = blockIdx.x;
-  if (threadIdx.x < 32) {
-    const int lane = threadIdx.x;
-    int n = 0;
-    for (int j0 = 0; j0 < top_k; j0 += 32) {
-      const int j = j0 + lane;
-      const int row = (j < top_k) ? row_of_slot[t * top_k + j] : -1;
-      const float w = (row >= 0) ? topk_w[t * top_k + j] : 0.f;
-      const unsigned m = __ballot_sync(0xffffffffu, row >= 0);
-      if (row >= 0) {
-        const int p = n + __popc(m & ((1u << lane) - 1u));
-        s_row[p] = row;
-        s_w[p] = w;
-      }
-      n += __popc(m);
-    }
-    if (lane == 0) s_n = n;
-  }
-  __syncthreads();
-  const int n = s_n;
-  for (int h0 = threadIdx.x * 4; h0 < H; h0 += 1024 * HV) {
-    float4 acc[HV];
-#pragma unroll
-    for (int u = 0; u < HV; ++u) acc[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int j = 0; j < n; j += 2) {   // two routed experts per round: 2 x HV independent loads in flight per thread
-      const bool two = (j + 1 < n);
-      const float* yr0 = y + (size_t)s_row[j] * H + h0;
-      const float* yr1 = y + (size_t)s_row[two ? j + 1 : j] * H + h0;
-      const float w0 = s_w[j], w1 = two ? s_w[j + 1] : 0.f;
-      float4 v0[HV], v1[HV];
-#pragma unroll
-      for (int u = 0; u < HV; ++u) {
-        const bool in = (h0 + u * 1024 < H);
-        v0[u] = in ? __ldcs(reinterpret_cast<const float4*>(yr0 + u * 1024)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        v1[u] = (in && two) ? __ldcs(reinterpret_cast<const float4*>(yr1 + u * 1024)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int u = 0; u < HV; ++u) {
-        acc[u].x = fmaf(w0, v0[u].x, acc[u].x);
-        acc[u].y = fmaf(w0, v0[u].y, acc[u].y);
-        acc[u].z = fmaf(w0, v0[u].z, acc[u].z);
-        acc[u].w = fmaf(w0, v0[u].w, acc[u].w);
-      }
-      if (two) {
-#pragma unroll
-        for (int u = 0; u < HV; ++u) {
-          acc[u].x = fmaf(w1, v1[u].x, acc[u].x);
-          acc[u].y = fmaf(w1, v1[u].y, acc[u].y);
-          acc[u].z = fmaf(w1, v1[u].z, acc[u].z);
-          acc[u].w = fmaf(w1, v1[u].w, acc[u].w);
-        }
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < HV; ++u) {
-      const int h = h0 + u * 1024;
-      if (h >= H) break;
-      const size_t o = (size_t)t * H + h;
-      if (out_dtype == 2) {
-        *reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + o) = acc[u];
-      } else if (out_dtype == 0) {
-        __nv_bfloat162 a = __floats2bfloat162_rn(acc[u].x, acc[u].y), b = __floats2bfloat162_rn(acc[u].z, acc[u].w);
-        uint2 pk;
-        pk.x = *reinterpret_cast<uint32_t*>(&a);
-        pk.y = *reinterpret_cast<uint32_t*>(&b);
-        *reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(out) + o) = pk;
-      } else {
-        __half2 a = __floats2half2_rn(acc[u].x, acc[u].y), b = __floats2half2_rn(acc[u].z, acc[u].w);
-        uint2 pk;
-        pk.x = *reinterpret_cast<uint32_t*>(&a);
-        pk.y = *reinterpret_cast<uint32_t*>(&b);
-        *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(out) + o) = pk;
-      }
-    }
-  }
-}
-
 static int64_t rows_bound(int64_t slots, int E) {
   const int64_t act = slots < E ? slots : E;
   return ((slots + (ROW_ALIGN - 1) * act) + ROW_ALIGN - 1) / ROW_ALIGN * ROW_ALIGN;
@@ -583,16 +493,7 @@ int launch_prep(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const vo
 
 int launch_combine(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const float* topk_w, int M, int k,
                    void* out, int out_dtype) {
-  // B200MOE_COMBINE=2 selects the compacted / register-resident form (bit-identical; opt-in until measured on hardware)
-  const char* cv = getenv("B200MOE_COMBINE");
-  if (cv && cv[0] == '2' && k <= 64) {
-    if (L->H <= 4096)
-      combine_v2_kernel<4><<<M, 256, 0, st>>>(ws->y, topk_w, ws->row_of_slot, k, L->H, out, out_dtype);
-    else
-      combine_v2_kernel<8><<<M, 256, 0, st>>>(ws->y, topk_w, ws->row_of_slot, k, L->H, out, out_dtype);
-  } else {
-    combine_kernel<<<M, 256, 0, st>>>(ws->y, topk_w, ws->row_of_slot, k, L->H, out, out_dtype);
-  }
+  combine_kernel<<<M, 256, 0, st>>>(ws->y, topk_w, ws->row_of_slot, k, L->H, out, out_dtype);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "combine launch");
@@ -664,8 +565,6 @@ int ensure_workspace(Workspace* ws, const b200moe_layer* L, int64_t tokens, int 
     WS_ALLOC(ws->partials, (int64_t)(4 * 160 * 2 + 160 * 4) * (2 * 64 * 128) * 4);
     WS_ALLOC(ws->fsync, (int64_t)sizeof(FusedSync));
     cudaMemset(ws->fsync, 0, sizeof(FusedSync));
-    WS_ALLOC(ws->dbg, (int64_t)160 * 16 * 8);
-    cudaMemset(ws->dbg, 0, 160 * 16 * 8);
   }
   cudaMemset(ws->state, 0, sizeof(RouteState));
   // the fresh buffers are first touched by work enqueued after this point; the legacy-stream memsets above are
@@ -735,7 +634,7 @@ void release_workspace(Workspace* ws) {
                   reinterpret_cast<void**>(&ws->state), reinterpret_cast<void**>(&ws->xt), reinterpret_cast<void**>(&ws->xs),
                   reinterpret_cast<void**>(&ws->it), reinterpret_cast<void**>(&ws->is), reinterpret_cast<void**>(&ws->y),
                   reinterpret_cast<void**>(&ws->partials), reinterpret_cast<void**>(&ws->fsync),
-                  reinterpret_cast<void**>(&ws->dbg), &ws->d_hidden, reinterpret_cast<void**>(&ws->d_ids),
+                  &ws->d_hidden, reinterpret_cast<void**>(&ws->d_ids),
                   reinterpret_cast<void**>(&ws->d_w), reinterpret_cast<void**>(&ws->d_out),
                   reinterpret_cast<void**>(&ws->dq13), reinterpret_cast<void**>(&ws->dq2)};
   for (void** p : cur) {
@@ -748,7 +647,6 @@ void release_workspace(Workspace* ws) {
   ws->cap_stage_tokens = ws->cap_stage_k = 0;
   ws->cap_dq13 = ws->cap_dq2 = 0;
   ws->bytes = 0;
-  ws->dbg_enabled = false;
 }
 
 }  // namespace b200

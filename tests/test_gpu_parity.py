@@ -418,6 +418,11 @@ def test_mla_decode_vs_oracle(dev, B, S, page, Hq):
     # metric + thresholds of reference tests/kernels/attention/test_cutlass_mla_decode.py:15-32
     assert _cos_diff(out.cpu().float(), ref) < 1e-5
     torch.testing.assert_close(lse.cpu(), lse_ref, atol=1e-3, rtol=1e-3)
+    from lvllm_b200._lib import B200Error
+    with pytest.raises(B200Error, match="num_heads <= 128"):   # one head more than the kernel serves
+        ops.mla_decode(torch.zeros(B, 129, 512, dtype=torch.bfloat16, device=dev),
+                       torch.zeros(B, 129, 64, dtype=torch.bfloat16, device=dev), cache.to(dev), lens.to(dev), pt.to(dev),
+                       scale)
 
 
 @pytest.mark.parametrize("splits", [0, 3])   # 0: tensor-core path (128-token splits); 3: CUDA-core split-KV path
