@@ -226,6 +226,19 @@ int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const v
                        int64_t page_stride, int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table,
                        int batch, int num_q_heads, int num_kv_heads, int head_dim, int page_size, int max_pages,
                        float sm_scale, int num_splits, void* workspace, void* out, float* lse);
+/* Speculative-decode verification: the arguments of b200_gqa_decode_ex plus q_len = Q query tokens per request (uniform
+ * over the batch, 1 <= Q <= 16; B200_ERR_INVALID otherwise, nothing launched).  q [B*Q, Hq, D] bf16 with request b's Q
+ * tokens contiguous in draft order (vLLM's decode_query layout); seq_lens[b] = S_b counts all of request b's keys, its Q
+ * new tokens included (written to the cache before this call).  Query token i of request b attends to key positions
+ * [0, S_b - Q + i] (the end-aligned causal mask of a multi-token decode, reference tests/kernels/attention/
+ * test_flashinfer.py:29-80 with query_lens = [Q] * B).  out bf16 [B*Q, Hq, D], lse f32 [B*Q, Hq] (natural log) or NULL,
+ * row (b * Q + i, h); a row with no visible key (S_b - Q + 1 + i <= 0) gives out = 0, lse = -inf.  The workspace is
+ * b200_gqa_decode_workspace_bytes(batch * q_len, num_q_heads, head_dim, num_splits) bytes.  q_len = 1 is
+ * b200_gqa_decode_ex. */
+int b200_gqa_decode_spec(void* stream, const void* q, const void* k_cache, const void* v_cache, int64_t block_stride,
+                         int64_t page_stride, int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table,
+                         int batch, int q_len, int num_q_heads, int num_kv_heads, int head_dim, int page_size,
+                         int max_pages, float sm_scale, int num_splits, void* workspace, void* out, float* lse);
 /* The GQA decode kernel's neighbour, bf16: one launch per step for what the reference runs as Qwen3's per-head q/k RMSNorm
  * (models/qwen3_moe.py:333-351) + RoPE (fused_qk_norm_rope, vllm/_custom_ops.py:279; rotary_embedding/base.py:161-201)
  * + reshape_and_cache_flash (csrc/libtorch_stable/cache_kernels.cu:315-400, called at flashinfer.py:2276-2290).

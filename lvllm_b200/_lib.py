@@ -71,6 +71,8 @@ PROTOTYPES = {
                                _vp, _vp, _vp]),
     "b200_gqa_decode_ex": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _f32,
                                   _i32, _vp, _vp, _vp]),
+    "b200_gqa_decode_spec": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32,
+                                    _f32, _i32, _vp, _vp, _vp]),
     "b200_gqa_qknorm_rope_cache_write": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _vp, _vp, _i64,
                                                 _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32]),
     "b200_ep_flag_bytes": (_i64, []),

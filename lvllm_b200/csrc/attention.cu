@@ -1,5 +1,6 @@
-// Paged decode attention (one query token per request), split-KV + LSE merge: the entry points, the split merges and
-// the CUDA-core GQA kernel.
+// Paged decode attention, split-KV + LSE merge: the entry points, the split merges and the CUDA-core GQA kernel.
+// MLA takes one query token per request; GQA takes Q >= 1 (speculative decode: query token i of request b sees keys
+// [0, S_b - Q + i], the end-aligned causal mask).
 //   MLA (absorbed): q = [q_nope(512) | q_pe(64)], one shared latent KV head, K = all 576 cols, V = first 512
 //                   (op contract of reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262);
 //                   up to 128 heads, on the tensor-core kernel (attention_mla.cu)
@@ -13,6 +14,8 @@
 // head), so HBM traffic == algorithmic KV bytes; the warp does the dot product over its lane-strided dims,
 // online softmax in fp32 (exp2 domain), and accumulates V.  It serves groups of more than 32 query heads per kv head,
 // more work items per CTA than the tensor-core kernel's table holds, and split counts that do not cover the page table.
+// With Q query tokens per request each query row (b, i) is a CTA row of its own that does exactly the arithmetic of a
+// single-token decode over its S_b - Q + 1 + i keys, so this path reads a request's KV Q times (acceptable for a fallback).
 // Partial (o, m, l) per split are merged by a second tiny kernel that also emits the natural-log LSE.
 // Roofline: HBM (KV bytes).
 #include <math_constants.h>
@@ -30,8 +33,8 @@ __global__ void __launch_bounds__(WARPS * 32)
                        const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ seq_lens,
                        const int32_t* __restrict__ page_table, int Hq, int Hkv, int page_size, int max_pages,
                        float scale_log2, int num_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
-                       int64_t block_stride, int64_t page_stride, int64_t head_stride) {
-  // blockIdx.x = ((b * Hkv + hkv) * groups_per_kv + hg), blockIdx.y = split
+                       int64_t block_stride, int64_t page_stride, int64_t head_stride, int Q) {
+  // blockIdx.x = (((b * Q + i) * Hkv + hkv) * groups_per_kv + hg) for draft token i, blockIdx.y = split
   // K / V row of (page, slot in page, kv head) at page * block_stride + slot * page_stride + hkv * head_stride (elements)
   const int G = Hq / Hkv;
   const int groups_per_kv = (G + WARPS - 1) / WARPS;
@@ -39,14 +42,15 @@ __global__ void __launch_bounds__(WARPS * 32)
   const int hg = bx % groups_per_kv;
   bx /= groups_per_kv;
   const int hkv = bx % Hkv;
-  const int b = bx / Hkv;
+  const int row = bx / Hkv;   // query row b * Q + i
+  const int b = row / Q;
   const int split = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int head_in_group = hg * WARPS + warp;
   const bool head_ok = head_in_group < G;
   const int hq = hkv * G + (head_ok ? head_in_group : 0);
 
-  const int S = seq_lens[b];
+  const int S = max(seq_lens[b] - Q + 1 + row % Q, 0);   // keys this query token sees
   const int per = ((S + num_splits - 1) / num_splits + ATT_TOK - 1) / ATT_TOK * ATT_TOK;
   const int s0 = split * per;
   const int s1 = min(S, s0 + per);
@@ -57,7 +61,7 @@ __global__ void __launch_bounds__(WARPS * 32)
   constexpr int NK = DK / 32, NV = DV / 32;
   float qr[NK];
 #pragma unroll
-  for (int i = 0; i < NK; ++i) qr[i] = __bfloat162float(q[((size_t)b * Hq + hq) * DK + lane + 32 * i]) * scale_log2;
+  for (int i = 0; i < NK; ++i) qr[i] = __bfloat162float(q[((size_t)row * Hq + hq) * DK + lane + 32 * i]) * scale_log2;
   float o[NV];
 #pragma unroll
   for (int i = 0; i < NV; ++i) o[i] = 0.f;
@@ -120,7 +124,7 @@ __global__ void __launch_bounds__(WARPS * 32)
     }
   }
   if (head_ok) {
-    const size_t base = ((size_t)b * Hq + hq) * num_splits + split;
+    const size_t base = ((size_t)row * Hq + hq) * num_splits + split;
 #pragma unroll
     for (int i = 0; i < NV; ++i) part_o[base * DV + lane + 32 * i] = o[i];
     if (lane == 0) {
@@ -274,6 +278,19 @@ int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const v
                        int64_t page_stride, int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table,
                        int batch, int num_q_heads, int num_kv_heads, int head_dim, int page_size, int max_pages,
                        float sm_scale, int num_splits, void* workspace, void* out, float* lse) {
+  return b200_gqa_decode_spec(stream, q, k_cache, v_cache, block_stride, page_stride, head_stride, seq_lens, page_table,
+                              batch, 1, num_q_heads, num_kv_heads, head_dim, page_size, max_pages, sm_scale, num_splits,
+                              workspace, out, lse);
+}
+
+int b200_gqa_decode_spec(void* stream, const void* q, const void* k_cache, const void* v_cache, int64_t block_stride,
+                         int64_t page_stride, int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table,
+                         int batch, int q_len, int num_q_heads, int num_kv_heads, int head_dim, int page_size,
+                         int max_pages, float sm_scale, int num_splits, void* workspace, void* out, float* lse) {
+  if (q_len < 1 || q_len > 16) {
+    set_error("b200_gqa_decode: q_len must be in [1, 16]");
+    return B200_ERR_INVALID;
+  }
   if (!q || !k_cache || !v_cache || !seq_lens || !page_table || !workspace || !out || batch <= 0 ||
       num_q_heads <= 0 || num_kv_heads <= 0 || num_q_heads % num_kv_heads || page_size <= 0 || num_splits <= 0) {
     set_error("b200_gqa_decode: bad argument");
@@ -292,23 +309,25 @@ int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const v
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int G = num_q_heads / num_kv_heads;
   float* po = reinterpret_cast<float*>(workspace);
-  float* pml = po + (size_t)batch * num_q_heads * num_splits * 128;
+  const int rows = batch * q_len;   // query rows (b, i), b * q_len + i
+  float* pml = po + (size_t)rows * num_q_heads * num_splits * 128;
   const float sl2 = sm_scale * 1.4426950408889634f;
-  // tensor-core path (persistent CTAs over (request, kv head, 128-token split) items): needs the split count
+  // tensor-core path (persistent CTAs over (request, kv head, q-group, 128-token split) items): needs the split count
   // to cover the longest sequence the page table can describe
   if (G <= 128 && num_splits <= 1024 && (int64_t)num_splits * 128 >= (int64_t)max_pages * page_size) {
     const int rc = launch_gqa_tc(st, q, k_cache, v_cache, block_stride, page_stride, head_stride, seq_lens, page_table, batch,
-                                 num_q_heads, num_kv_heads, page_size, max_pages, sm_scale, num_splits, po, pml, out, lse);
+                                 q_len, num_q_heads, num_kv_heads, page_size, max_pages, sm_scale, num_splits, po, pml, out,
+                                 lse);
     if (rc <= 0) return rc;   // rc == 1: more work items per CTA than the kernel's table holds
   }
 #define LAUNCH_GQA(W)                                                                                          \
   {                                                                                                            \
     const int groups = (G + W - 1) / W;                                                                        \
-    dim3 grid(batch * num_kv_heads * groups, num_splits);                                                      \
+    dim3 grid(rows * num_kv_heads * groups, num_splits);                                                       \
     decode_attn_kernel<128, 128, W><<<grid, W * 32, 0, st>>>(                                                  \
         reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(k_cache),            \
         reinterpret_cast<const __nv_bfloat16*>(v_cache), seq_lens, page_table, num_q_heads, num_kv_heads,      \
-        page_size, max_pages, sl2, num_splits, po, pml, block_stride, page_stride, head_stride);               \
+        page_size, max_pages, sl2, num_splits, po, pml, block_stride, page_stride, head_stride, q_len);        \
   }
   if (G <= 4)
     LAUNCH_GQA(4)
@@ -317,8 +336,8 @@ int b200_gqa_decode_ex(void* stream, const void* q, const void* k_cache, const v
   else
     LAUNCH_GQA(16)
 #undef LAUNCH_GQA
-  decode_merge_kernel<128><<<(batch * num_q_heads + 3) / 4, 128, 0, st>>>(
-      po, pml, batch * num_q_heads, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
+  decode_merge_kernel<128><<<(rows * num_q_heads + 3) / 4, 128, 0, st>>>(
+      po, pml, rows * num_q_heads, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
   g_launches += 2;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "gqa_decode launch");

@@ -1,8 +1,13 @@
 // Paged GQA decode on wgmma tensor cores (head_dim 128), persistent CTAs, multi-stage KV pipeline.
 //
-// Work item = (request b, kv head, 128-token split).  The kernel is KV-bandwidth bound, so the tiles are laid
+// Work item = (request b, kv head, q-group, 128-token split).  The kernel is KV-bandwidth bound, so the tiles are laid
 // out to make every thread useful: tokens are the M rows of the MMAs and the G = Hq/Hkv query heads sharing the
-// kv head are the N columns (N = G rounded up to 16):
+// kv head are the N columns (N = G rounded up to 16).
+// Speculative decode: a request has Q query tokens (its last Q positions, in draft order); query token i sees keys
+// [0, S_b - Q + i] (end-aligned causal mask).  A q-group holds Qg = min(Q, 32 / G) of them: column c of the item is
+// (draft token qg * Qg + c / G, head c % G), N = G * Qg rounded up to 16, so while G * Q <= 32 K and V are read once per
+// request; beyond that every q-group reads them again.  Q = 1 is the single-token decode (one q-group, columns = heads).
+// The MMAs below, per item:
 //   S^T[128 tokens, N]  = K[128 tokens, 128 dims] . Q^T           (A = K tile, K-major; B = Q rows, K-major)
 //   P^T = exp2(S^T * scale - m)                                    (thread = token; m via warp shuffles)
 //   O^T[128 dims, N]    = V^T[128 dims, 128 tokens] . P^T          (A = V tile read MN-major; B = P rows, K-major)
@@ -14,7 +19,7 @@
 // softmax / epilogue threads through the exchange area (common.cuh), S^T double-buffered so that QK^T of item n+1
 // overlaps softmax of item n.  Partial (O, m, l) per split are merged by attn_merge_kernel.
 // Reference semantics: tests/kernels/attention/test_flashinfer.py:29-80 (ref_paged_attn, decode case).
-// Roofline: HBM — algorithmic bytes = sum_b S_b * Hkv * 128 * 2 (K and V) * 2 B.
+// Roofline: HBM — algorithmic bytes = sum_b S_b * Hkv * 128 * 2 (K and V) * 2 B * n_qg (n_qg = ceil(Q / Qg) q-groups).
 #include <math_constants.h>
 #include <stdio.h>
 
@@ -36,7 +41,10 @@ struct GqaBars {
   uint64_t s_full[2], p_full[2], o_full[2], o_done[2];
   float lsum[2][GQA_MAX_N];        // row sums of P per head (the rows of L are all the same: one is kept)
   alignas(16) float wmax[2][4][GQA_MAX_N];
-  int16_t nt_tab[GQA_MAX_ITEMS];   // valid tokens of this CTA's i-th item (<= 0: empty split)
+  int16_t nt_tab[GQA_MAX_ITEMS];   // valid tokens of this CTA's i-th item (<= 0: empty split): those of its last column
+  int16_t vis_tab[GQA_MAX_ITEMS];  // v of the i-th item: local draft token j of the q-group sees split tokens t <= v + j
+                                   // (clamped to [-32, 128], which keeps every mask the same)
+  int col_row[GQA_MAX_N];          // output row of column c relative to the item's first: (c / G) * Hq + c % G
 };
 
 // intra-CTA mbarrier wait (producer / MMA / softmax warps of ONE CTA: no other CTA or GPU is waited for).  A protocol bug
@@ -55,15 +63,17 @@ B200_DEVICE float ex2_approx(float v) {
 }
 B200_DEVICE void bar_sync_group(int g) { asm volatile("bar.sync %0, 128;" ::"r"(g + 1) : "memory"); }
 
+// SPEC: Q > 1 query tokens per request.  Without it every q-group expression below is a compile-time constant (Q = Qg = 1,
+// columns = heads), which keeps the single-token decode free of the per-column bookkeeping.
 // smem: [ones 1 KB][P group 0 | P group 1: 2 x N x 128 B each][stage: Q (2 x N x 128 B) | K 32 KB | V 32 KB] x NST
 //       [exchange: 2 groups x N columns x 512 B][bars]
-template <int N>
+template <int N, bool SPEC>
 __global__ void __launch_bounds__(GQA_THREADS, 1)
     gqa_decode_tc_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
                          const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ seq_lens,
                          int64_t block_stride, int64_t page_stride, int64_t head_stride,
                          const int32_t* __restrict__ page_table, int B, int Hq, int Hkv, int page_size, int max_pages,
-                         float scale_log2, int num_splits, int NST, float* __restrict__ part_o,
+                         float scale_log2, int num_splits, int Q_, int Qg_, int NST, float* __restrict__ part_o,
                          float* __restrict__ part_ml) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -77,7 +87,11 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
   GqaBars* bars = reinterpret_cast<GqaBars*>(xch_area + 2 * N * 512);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int G = Hq / Hkv;
-  const int total = B * Hkv * num_splits;
+  const int Q = SPEC ? Q_ : 1, Qg = SPEC ? Qg_ : 1;
+  const int n_qg = SPEC ? (Q + Qg - 1) / Qg : 1;
+  const int total = B * Hkv * n_qg * num_splits;
+  // item = ((b * Hkv + kvh) * n_qg + qg) * num_splits + split; its rows (b * Q + qg * Qg + c / G, kvh * G + c % G) start at
+  // row0 = (b * Q + qg * Qg) * Hq + kvh * G and it has ncols = G * (number of draft tokens of the q-group) columns
 
   if (tid == 0) {
     for (int i = 0; i < GQA_MAX_STAGES; ++i) {
@@ -96,9 +110,14 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
   const int my_items = blockIdx.x < total ? (total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   for (int i = tid; i < my_items; i += GQA_THREADS) {
     const int item = blockIdx.x + i * gridDim.x;
-    const int left = seq_lens[item / (num_splits * Hkv)] - (item % num_splits) * GQA_TOK;
-    bars->nt_tab[i] = (int16_t)max(0, min(GQA_TOK, left));
+    const int rest = item / num_splits, qg = rest % n_qg;
+    const int qn = min(Qg, Q - qg * Qg);
+    const int v = seq_lens[rest / (n_qg * Hkv)] - Q + qg * Qg - (item % num_splits) * GQA_TOK;
+    bars->nt_tab[i] = (int16_t)max(0, min(GQA_TOK, v + qn));
+    if (SPEC) bars->vis_tab[i] = (int16_t)max(-32, min(GQA_TOK, v));
   }
+  if (SPEC && tid < GQA_MAX_N) bars->col_row[tid] = (tid / G) * Hq + tid % G;
+  auto col_row = [&](int c) { return SPEC ? bars->col_row[c] : c; };
   if (tid < 64) reinterpret_cast<uint4*>(ones)[tid] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
   fence_proxy_async();
   __syncthreads();
@@ -113,7 +132,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
     auto lookup = [&](int i, int* out) {
       if (i >= my_items) return;
       const int item = blockIdx.x + i * gridDim.x;
-      const int split = item % num_splits, b = item / (num_splits * Hkv);
+      const int split = item % num_splits, b = item / (num_splits * n_qg * Hkv);
 #pragma unroll
       for (int u = 0; u < 8; ++u) {
         const int pi = min((split * GQA_TOK + r0 + 16 * u) / page_size, max_pages - 1);
@@ -127,15 +146,18 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       const int nt = bars->nt_tab[i];
       if (nt > 0) {
         const int item = blockIdx.x + i * gridDim.x;
-        const int split = item % num_splits, kvh = (item / num_splits) % Hkv, b = item / (num_splits * Hkv);
+        const int split = item % num_splits, rest = item / num_splits, qg = rest % n_qg, kvh = (rest / n_qg) % Hkv,
+                  b = rest / (n_qg * Hkv);
+        const int ncols = SPEC ? G * min(Qg, Q - qg * Qg) : G;
+        const __nv_bfloat16* qrow0 = q + ((size_t)(b * Q + qg * Qg) * Hq + kvh * G) * 128 + c * 8;
         const int s = n % NST;
         uint8_t* q_t = stages + (size_t)s * stage_bytes;
         uint8_t* k_t = q_t + 2 * qbytes;
         uint8_t* v_t = k_t + 2 * TILE_BYTES;
         gqa_wait(&bars->kv_free[s], ((n / NST) & 1) ^ 1);
         for (int r = r0; r < N; r += 16) {
-          const bool qok = r < G;
-          const __nv_bfloat16* src = q + ((size_t)b * Hq + kvh * G + (qok ? r : 0)) * 128 + c * 8;
+          const bool qok = r < ncols;
+          const __nv_bfloat16* src = qrow0 + (size_t)(qok ? col_row(r) : 0) * 128;
           cp_async16(q_t + sw128_offset(r, c * 16), src, qok);
           cp_async16(q_t + qbytes + sw128_offset(r, c * 16), src + 64, qok);
         }
@@ -246,12 +268,15 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
     for (int i = 0; i < my_items; ++i) {
       const int nt = bars->nt_tab[i];
       const int item = blockIdx.x + i * gridDim.x;
-      const int split = item % num_splits, kvh = (item / num_splits) % Hkv, b = item / (num_splits * Hkv);
-      const size_t pbase = ((size_t)b * Hq + kvh * G) * num_splits + split;   // + h * num_splits
+      const int split = item % num_splits, rest = item / num_splits, qg = rest % n_qg, kvh = (rest / n_qg) % Hkv,
+                b = rest / (n_qg * Hkv);
+      const int ncols = SPEC ? G * min(Qg, Q - qg * Qg) : G;
+      const size_t pbase = ((size_t)(b * Q + qg * Qg) * Hq + kvh * G) * num_splits + split;   // + col_row[c] * num_splits
       if (nt <= 0) {
-        if (g == 0 && t < G) {
-          part_ml[(pbase + (size_t)t * num_splits) * 2] = -CUDART_INF_F;
-          part_ml[(pbase + (size_t)t * num_splits) * 2 + 1] = 0.f;
+        if (g == 0 && t < ncols) {
+          const size_t r = pbase + (size_t)col_row(t) * num_splits;
+          part_ml[r * 2] = -CUDART_INF_F;
+          part_ml[r * 2 + 1] = 0.f;
         }
         continue;
       }
@@ -260,6 +285,8 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
         continue;
       }
       const uint32_t ph = (n >> 1) & 1;
+      // token t is visible to the columns c >= cmin (those of draft tokens j >= t - v); t >= nt: to none of the item's
+      const int cmin = SPEC ? max(t - bars->vis_tab[i], 0) * G : 0;
       const bool tv = t < nt;
       gqa_wait(&bars->s_full[g], ph);
       float my_ms = 0.f;                          // thread t == h keeps m[h] * scale for the partial record
@@ -269,7 +296,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
         xch_ld<16>(tm_s + c0, v);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          v[j] = tv ? v[j] : -CUDART_INF_F;
+          v[j] = (SPEC ? c0 + j >= cmin : tv) ? v[j] : -CUDART_INF_F;
           const float wm = warp_max(v[j]);
           if (lane == j) wmax[warp & 3][c0 + j] = wm;
         }
@@ -291,7 +318,9 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
         for (int j = 0; j < 16; ++j) {
           const float ms = m[j] * scale_log2;
           my_ms = (t == c0 + j) ? ms : my_ms;
-          const float p = ex2_approx(fmaf(v[j], scale_log2, -ms));      // masked tokens: ex2(-inf) = 0
+          // masked tokens: ex2(-inf) = 0; a column with no visible token in this split (m = -inf) gets P = 0, l = 0 and
+          // records m = -inf, which the merge skips
+          const float p = SPEC && m[j] == -CUDART_INF_F ? 0.f : ex2_approx(fmaf(v[j], scale_log2, -ms));
           *reinterpret_cast<__nv_bfloat16*>(pr + (j >> 3) * 1024 + (j & 7) * 128 + ((bch ^ (j & 7)) << 4) + blo) =
               __float2bfloat16_rn(p);
         }
@@ -309,11 +338,12 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
         xch_ld<16>(tm_o + c0, o);
 #pragma unroll
         for (int j = 0; j < 16; ++j)
-          if (c0 + j < G) po[(size_t)(c0 + j) * hstride] = o[j];
+          if (c0 + j < ncols) po[(size_t)col_row(c0 + j) * hstride] = o[j];
       }
-      if (t < G) {
-        part_ml[(pbase + (size_t)t * num_splits) * 2] = my_ms;
-        part_ml[(pbase + (size_t)t * num_splits) * 2 + 1] = bars->lsum[g][t];
+      if (t < ncols) {
+        const size_t r = pbase + (size_t)col_row(t) * num_splits;
+        part_ml[r * 2] = my_ms;
+        part_ml[r * 2 + 1] = bars->lsum[g][t];
       }
       mbar_arrive(&bars->o_done[g]);   // the group's columns and row sums may be overwritten
       ++n;
@@ -380,15 +410,16 @@ __global__ void __launch_bounds__(DV / 4) attn_merge_kernel(const float* __restr
 }
 
 int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc, int64_t block_stride, int64_t page_stride,
-                  int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table, int batch, int Hq, int Hkv,
-                  int page_size, int max_pages, float sm_scale, int num_splits, float* part_o, float* part_ml, void* out,
-                  float* lse) {
+                  int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table, int batch, int q_len, int Hq,
+                  int Hkv, int page_size, int max_pages, float sm_scale, int num_splits, float* part_o, float* part_ml,
+                  void* out, float* lse) {
   static bool attr = false;
   static int num_sms = 0;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(gqa_decode_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, GQA_SMEM_MAX);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gqa_decode_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, GQA_SMEM_MAX);
+    cudaError_t e = cudaSuccess;
+    for (auto k : {gqa_decode_tc_kernel<16, false>, gqa_decode_tc_kernel<32, false>, gqa_decode_tc_kernel<16, true>,
+                   gqa_decode_tc_kernel<32, true>})
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, GQA_SMEM_MAX);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(gqa_decode_tc)");
     int dev = 0;
     cudaGetDevice(&dev);
@@ -396,9 +427,10 @@ int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc
     attr = true;
   }
   const int G = Hq / Hkv;
-  const int N = (G + 15) / 16 * 16;
+  if (G > GQA_MAX_N) return 1;   // not handled here
+  const int Qg = min(q_len, GQA_MAX_N / G), n_qg = (q_len + Qg - 1) / Qg;   // draft tokens per q-group, q-groups
+  const int N = (G * Qg + 15) / 16 * 16;
   const int qbytes = N * 128;
-  if (N > GQA_MAX_N) return 1;   // not handled here
   const int fixed = 1024 /*align*/ + 1024 /*ones*/ + 2 * ((2 * qbytes + 1023) & ~1023) + 2 * N * 512 /*exchange*/ +
                     (int)sizeof(GqaBars) + 64;
   const int stage_bytes = 2 * qbytes + 4 * TILE_BYTES;
@@ -413,15 +445,16 @@ int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc
     return B200_ERR_INVALID;
   }
   const int smem = fixed + nst * stage_bytes;
-  const int total = batch * Hkv * num_splits;
+  const int total = batch * Hkv * n_qg * num_splits;
   const int grid = total < num_sms ? total : num_sms;
   if ((total + grid - 1) / grid > GQA_MAX_ITEMS) return 1;   // not handled here: caller uses the split-KV CUDA-core path
-  auto kern = N == 16 ? gqa_decode_tc_kernel<16> : gqa_decode_tc_kernel<32>;
+  auto kern = q_len > 1 ? (N == 16 ? gqa_decode_tc_kernel<16, true> : gqa_decode_tc_kernel<32, true>)
+                        : (N == 16 ? gqa_decode_tc_kernel<16, false> : gqa_decode_tc_kernel<32, false>);
   kern<<<grid, GQA_THREADS, smem, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(kc),
       reinterpret_cast<const __nv_bfloat16*>(vc), seq_lens, block_stride, page_stride, head_stride, page_table, batch, Hq, Hkv, page_size, max_pages,
-      sm_scale * 1.4426950408889634f, num_splits, nst, part_o, part_ml);
-  attn_merge_kernel<128><<<batch * Hq, 32, 0, st>>>(part_o, part_ml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
+      sm_scale * 1.4426950408889634f, num_splits, q_len, Qg, nst, part_o, part_ml);
+  attn_merge_kernel<128><<<batch * q_len * Hq, 32, 0, st>>>(part_o, part_ml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
   g_launches += 2;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "gqa_decode_tc launch");

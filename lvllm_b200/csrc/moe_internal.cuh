@@ -157,9 +157,9 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
                   int num_splits, float* part_o, float* part_ml, int kv_fp8 = 0, int q_fp8 = 0, float descale_q = 1.f,
                   float descale_k = 1.f);
 int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc, int64_t block_stride, int64_t page_stride,
-                  int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table, int batch, int Hq, int Hkv,
-                  int page_size, int max_pages, float sm_scale, int num_splits, float* part_o, float* part_ml, void* out,
-                  float* lse);
+                  int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table, int batch, int q_len, int Hq,
+                  int Hkv, int page_size, int max_pages, float sm_scale, int num_splits, float* part_o, float* part_ml,
+                  void* out, float* lse);
 bool fused_supported(const b200moe_layer* L, int M, int k);
 int launch_fused(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const void* hidden, const int32_t* ids,
                  const float* topk_w, int M, int k, void* out, int out_dtype);

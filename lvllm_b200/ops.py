@@ -271,8 +271,13 @@ def _kv_cache_strides(k_cache: torch.Tensor, v_cache: torch.Tensor) -> tuple[int
 
 
 def gqa_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, seq_lens: torch.Tensor,
-               page_table: torch.Tensor, sm_scale: float, num_kv_splits: int = 0, max_seq_len: int | None = None):
-    """Paged GQA decode (q [B,Hq,128] bf16; caches [pages,page,Hkv,128] bf16 views).  Returns (out, lse).
+               page_table: torch.Tensor, sm_scale: float, num_kv_splits: int = 0, max_seq_len: int | None = None,
+               q_len_per_req: int = 1):
+    """Paged GQA decode (q [B*Q,Hq,128] bf16; caches [pages,page,Hkv,128] bf16 views).  Returns (out, lse), [B*Q,Hq,128]
+    and [B*Q,Hq].  B = seq_lens.numel(); Q = ``q_len_per_req`` query tokens per request (speculative-decode verification,
+    the reference decode path's q_len_per_req, flashinfer.py:2183-2188): request b's Q tokens are contiguous in draft
+    order, seq_lens[b] counts all its keys including the Q new ones, and token i attends to keys [0, seq_lens[b] - Q + i]
+    (a row with no visible key gives out 0 and lse -inf).  Q = 1 (the default) is the single-token decode.
     The caches are read in place through their own strides: separate contiguous caches, or the K / V halves of the
     FlashInfer backend's packed NHD / HND cache exactly as the backend hands them out (kv_cache.transpose(1, 2)
     .split(128, -1)); the head dim must be contiguous and the other strides multiples of 8 elements (ValueError otherwise).
@@ -281,10 +286,16 @@ def gqa_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, se
     qq = _cuda(q, "q")
     assert qq.dtype == torch.bfloat16
     bstride, pstride, hstride = _kv_cache_strides(k_cache, v_cache)
-    B, Hq, D = qq.shape
+    T, Hq, D = qq.shape
+    Q = int(q_len_per_req)
     page, Hkv = k_cache.shape[1], k_cache.shape[2]
-    sl = _cuda(seq_lens.to(torch.int32), "seq_lens")
+    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
     pt = _cuda(page_table.to(torch.int32), "page_table")
+    B = sl.numel()
+    if T != B * Q:
+        raise ValueError(f"q must hold q_len_per_req = {Q} tokens per request: {B * Q} rows for {B} seq_lens, got {T}")
+    if pt.dim() != 2 or pt.shape[0] != B:
+        raise ValueError(f"page_table must have one row per request ({B}), got {tuple(pt.shape)}")
     if max_seq_len is not None:
         max_pages = max(1, min(pt.shape[1], -(-int(max_seq_len) // page)))
         if max_pages != pt.shape[1]:
@@ -294,12 +305,12 @@ def gqa_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, se
         num_kv_splits = max(1, -(-(pt.shape[1] * page) // 128))
         if num_kv_splits > 1024:
             num_kv_splits = max(1, min(32, 592 // max(1, B * Hkv)))
-    ws = torch.empty(L.lib().b200_gqa_decode_workspace_bytes(B, Hq, D, num_kv_splits), dtype=torch.uint8, device=qq.device)
-    out = torch.empty(B, Hq, D, dtype=torch.bfloat16, device=qq.device)
-    lse = torch.empty(B, Hq, dtype=torch.float32, device=qq.device)
-    rc = L.lib().b200_gqa_decode_ex(_stream(), qq.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), bstride, pstride,
-                                    hstride, sl.data_ptr(), pt.data_ptr(), B, Hq, Hkv, D, page, pt.shape[1], float(sm_scale),
-                                    num_kv_splits, ws.data_ptr(), out.data_ptr(), lse.data_ptr())
+    ws = torch.empty(L.lib().b200_gqa_decode_workspace_bytes(T, Hq, D, num_kv_splits), dtype=torch.uint8, device=qq.device)
+    out = torch.empty(T, Hq, D, dtype=torch.bfloat16, device=qq.device)
+    lse = torch.empty(T, Hq, dtype=torch.float32, device=qq.device)
+    rc = L.lib().b200_gqa_decode_spec(_stream(), qq.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), bstride, pstride,
+                                      hstride, sl.data_ptr(), pt.data_ptr(), B, Q, Hq, Hkv, D, page, pt.shape[1],
+                                      float(sm_scale), num_kv_splits, ws.data_ptr(), out.data_ptr(), lse.data_ptr())
     L.check(rc, "b200_gqa_decode")
     return out, lse
 
