@@ -192,6 +192,24 @@ int b200_mla_decode_ex(void* stream, const void* q_nope, const void* q_pe, int q
                        int kv_dtype, float descale_q, float descale_k, const int32_t* seq_lens,
                        const int32_t* page_table, int batch, int num_heads, int page_size, int max_pages, float sm_scale,
                        int num_splits, void* workspace, void* out, float* lse);
+/* Speculative-decode verification (multi-token prediction): the arguments of b200_mla_decode_ex plus q_len = Q query
+ * tokens per request (uniform over the batch, 1 <= Q <= 16; B200_ERR_INVALID otherwise, nothing launched) and the optional
+ * up-projection of b200_mla_decode_vup.  q_nope [B*Q, Hq, 512], q_pe [B*Q, Hq, 64] with request b's Q tokens contiguous in
+ * draft order; seq_lens[b] = S_b counts all of request b's keys, its Q new tokens included (written to the cache before this
+ * call).  Query token i of request b attends to key positions [0, S_b - Q + i]: the end-aligned causal mask of the
+ * reference's FlashMLA decode (QueryLenSupport.UNIFORM, v1/attention/backends/mla/flashmla.py:120; the query reshaped to
+ * [B, Q, Hq, D] by reshape_query_for_spec_decode, backends/utils.py:745-758, and the kernel called with causal=True,
+ * flashmla.py:284-344).  Rows are (b * Q + i, h): out bf16 [B*Q, Hq, 512], lse f32 [B*Q, Hq] (natural log) or NULL; a row
+ * with no visible key (S_b - Q + 1 + i <= 0) gives out = 0, lse = -inf.  w_uv == NULL: out is required.  w_uv != NULL
+ * ([Hq,512,128] bf16): the split merge is fused with the v up-projection as in b200_mla_decode_vup, out_v bf16
+ * [B*Q, Hq, 128] is required, out is the optional latent output and num_splits <= 512.  The workspace is
+ * b200_mla_decode_workspace_bytes(batch * q_len, num_heads, num_splits) bytes.  q_len = 1 is b200_mla_decode_ex
+ * (w_uv == NULL) or b200_mla_decode_vup. */
+int b200_mla_decode_spec(void* stream, const void* q_nope, const void* q_pe, int q_dtype, const void* kv_cache,
+                         int kv_dtype, float descale_q, float descale_k, const int32_t* seq_lens,
+                         const int32_t* page_table, int batch, int q_len, int num_heads, int page_size, int max_pages,
+                         float sm_scale, int num_splits, void* workspace, void* out, float* lse, const void* w_uv,
+                         void* out_v);
 /* The MLA decode kernel's neighbours (SURVEY.md 8f row 3), bf16:
  *  b200_mla_rope_cache_write  RoPE of q_pe [T,Hq,64] and k_pe [T,64] in place (rotary_embedding/base.py:161-201; cos_sin_cache
  *      bf16 [max_pos,64] = cos | sin; is_neox 0 = GPT-J pairs (DeepSeek), 1 = NeoX halves) fused with concat_and_cache_mla

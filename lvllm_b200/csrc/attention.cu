@@ -1,5 +1,5 @@
 // Paged decode attention, split-KV + LSE merge: the entry points, the split merges and the CUDA-core GQA kernel.
-// MLA takes one query token per request; GQA takes Q >= 1 (speculative decode: query token i of request b sees keys
+// MLA and GQA take Q >= 1 query tokens per request (speculative decode: query token i of request b sees keys
 // [0, S_b - Q + i], the end-aligned causal mask).
 //   MLA (absorbed): q = [q_nope(512) | q_pe(64)], one shared latent KV head, K = all 576 cols, V = first 512
 //                   (op contract of reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262);
@@ -241,24 +241,41 @@ int b200_mla_decode_ex(void* stream, const void* q_nope, const void* q_pe, int q
                        int kv_dtype, float descale_q, float descale_k, const int32_t* seq_lens,
                        const int32_t* page_table, int batch, int num_heads, int page_size, int max_pages, float sm_scale,
                        int num_splits, void* workspace, void* out, float* lse) {
-  if (!q_nope || !q_pe || !kv_cache || !seq_lens || !page_table || !workspace || !out || batch <= 0 ||
-      num_heads <= 0 || num_heads > 128 || page_size <= 0 || num_splits <= 0 || q_dtype < 0 || q_dtype > 1 ||
-      kv_dtype < 0 || kv_dtype > 1) {
-    set_error("b200_mla_decode: bad argument (num_heads <= 128)");
+  return b200_mla_decode_spec(stream, q_nope, q_pe, q_dtype, kv_cache, kv_dtype, descale_q, descale_k, seq_lens, page_table,
+                              batch, 1, num_heads, page_size, max_pages, sm_scale, num_splits, workspace, out, lse, nullptr,
+                              nullptr);
+}
+
+int b200_mla_decode_spec(void* stream, const void* q_nope, const void* q_pe, int q_dtype, const void* kv_cache,
+                         int kv_dtype, float descale_q, float descale_k, const int32_t* seq_lens,
+                         const int32_t* page_table, int batch, int q_len, int num_heads, int page_size, int max_pages,
+                         float sm_scale, int num_splits, void* workspace, void* out, float* lse, const void* w_uv,
+                         void* out_v) {
+  if (q_len < 1 || q_len > 16) {
+    set_error("b200_mla_decode: q_len must be in [1, 16]");
+    return B200_ERR_INVALID;
+  }
+  if (!q_nope || !q_pe || !kv_cache || !seq_lens || !page_table || !workspace || batch <= 0 || num_heads <= 0 ||
+      num_heads > 128 || page_size <= 0 || num_splits <= 0 || q_dtype < 0 || q_dtype > 1 || kv_dtype < 0 || kv_dtype > 1 ||
+      (w_uv ? (!out_v || num_splits > 512) : !out)) {
+    set_error("b200_mla_decode: bad argument (num_heads <= 128; out, or with w_uv out_v and num_splits <= 512)");
     return B200_ERR_INVALID;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int rows = batch * q_len;   // query rows (b, i), b * q_len + i
   float* po = reinterpret_cast<float*>(workspace);
-  float* pml = po + (size_t)batch * num_heads * num_splits * 512;
+  float* pml = po + (size_t)rows * num_heads * num_splits * 512;
   // each CTA walks ceil(tiles / num_splits) 128-token tiles (online softmax)
-  int rc = launch_mla_tc(st, q_nope, q_pe, kv_cache, seq_lens, page_table, batch, num_heads, page_size, max_pages,
+  int rc = launch_mla_tc(st, q_nope, q_pe, kv_cache, seq_lens, page_table, batch, q_len, num_heads, page_size, max_pages,
                          sm_scale, num_splits, po, pml, kv_dtype, q_dtype, descale_q, descale_k);
   if (rc) return rc;
-  if (num_splits <= 512)
-    mla_merge_kernel<<<batch * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
+  if (w_uv)   // split merge fused with the v up-projection (mla_aux.cu)
+    launch_mla_merge_vup(st, po, pml, rows, num_splits, num_heads, w_uv, out_v, out, lse);
+  else if (num_splits <= 512)
+    mla_merge_kernel<<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
   else
-    decode_merge_kernel<512><<<(batch * num_heads + 3) / 4, 128, 0, st>>>(po, pml, batch * num_heads, num_splits,
-                                                                         reinterpret_cast<__nv_bfloat16*>(out), lse);
+    decode_merge_kernel<512><<<(rows * num_heads + 3) / 4, 128, 0, st>>>(po, pml, rows * num_heads, num_splits,
+                                                                        reinterpret_cast<__nv_bfloat16*>(out), lse);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "mla merge launch");

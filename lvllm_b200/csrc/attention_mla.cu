@@ -5,7 +5,7 @@
 //   O[128 heads, 128 dims]   = P[128, 128 tokens] * V[128 tokens, 128]     (V = first 512 latent dims; this
 //                                                                          CTA owns one quarter of them)
 //
-// One CTA = (request, run of 128-token KV tiles, quarter of the 512 value dims).  A KV tile is loaded ONCE into
+// One CTA = (request, q-group, run of 128-token KV tiles, quarter of the 512 value dims).  A KV tile is loaded ONCE into
 // shared memory as nine [128 tokens x 128 B] blocks with the 128-byte swizzle: block kb is the K-major B
 // operand of the QK^T MMA for dims [64kb, 64kb+64) and — the same bytes, read through an MN-major
 // descriptor — the B operand of the PV MMA for value dims [64kb, 64kb+64).  Two consumer warpgroups take 64 heads
@@ -14,10 +14,19 @@
 // nor P touches shared memory.  A quarter of the value dims per CTA is what keeps both accumulators in registers.
 // Partial (O, m, l) per split are merged by mla_merge_kernel (attention.cu), by decode_merge_kernel above 512 splits.
 //
+// Speculative decode (multi-token-prediction verification): a request has Q query tokens (its last Q positions, in draft
+// order); query token i sees keys [0, S_b - Q + i] (the end-aligned causal mask, reference FlashMLA with causal=True,
+// v1/attention/backends/mla/flashmla.py:284-344).  The 128 MMA rows become (draft token, head) pairs: a q-group holds
+// Qg = min(Q, 128 / Hq) draft tokens and row r is draft token qg * Qg + r / Hq, head r % Hq, i.e. q / output row
+// (b * Q + qg * Qg) * Hq + r.  Rows past the group's last token load zero q and are never written.  The q-group index
+// varies with the value-dim part in blockIdx.y, so the CTAs reading the same KV tile are scheduled together.  Each
+// accumulator row masks with its own key count; Q = 1 is the single-token decode (one q-group, rows = heads).
+//
 // Warp roles (384 threads): warps 0-3 / 4-7 consumer warpgroups (MMA + softmax + epilogue), warps 8-11 loaders
 // (16-byte gathers of q rows / paged KV rows -> swizzled smem, generic->async proxy fence).
 // The op contract is reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262.
-// Roofline: KV bytes (HBM / L2) — at B=1 the kernel is latency bound.
+// Roofline: KV bytes (HBM / L2) — at B=1 the kernel is latency bound.  Algorithmic bytes = sum_b S_b * 576 * {2, 1} (bf16,
+// e4m3 cache) * n_qg (n_qg = ceil(Q / Qg) q-groups, each reading the request's tiles again).
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -38,6 +47,7 @@ constexpr int MLA_SMEM = MLA_K_AREA + MLA_Q_RING + 1024 + 1024;
 struct MlaBars {
   uint64_t full[MLA_KB], empty[MLA_QSTAGES];
   uint64_t s_full, o_full;   // QK^T / PV of the tile complete in both warpgroups: its blocks may be refilled
+  int8_t row_off[128];       // SPEC: MMA row r sees row_off[r] keys fewer than the q-group's last draft token
 };
 
 B200_DEVICE void mla_wait(uint64_t* bar, uint32_t parity) {
@@ -68,13 +78,15 @@ B200_DEVICE uint4 fp8x8_to_bf16x8(uint2 v) {
 // reference fp8 dtypes backends/mla/cutlass_mla.py:44-45).  The loaders widen it to bf16 on the way into shared memory
 // (exact), so the tensor-core pipeline and its numerics are those of the bf16 kernel — P is NOT re-quantised to fp8.
 // q8: the queries are e4m3 too (the reference's fp8 test feeds fp8 q, tests/kernels/attention/test_cutlass_mla_decode.py:101-110).
-template <bool KV8>
+// SPEC: Q > 1 query tokens per request.  Without it every q-group expression below is a compile-time constant (Q = Qg = 1,
+// rows = heads, one limit for every row), which keeps the single-token decode free of the per-row bookkeeping.
+template <bool KV8, bool SPEC>
 __global__ void __launch_bounds__(MLA_THREADS, 1)
     mla_decode_tc_kernel(const void* __restrict__ q_nope_v, const void* __restrict__ q_pe_v,
                          const void* __restrict__ kv_v, const int32_t* __restrict__ seq_lens,
                          const int32_t* __restrict__ page_table, int Hq, int page_size, int max_pages,
                          float scale_log2, int num_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
-                         int q8, float out_scale, int tiles_per_cta) {
+                         int q8, float out_scale, int tiles_per_cta, int Q_, int Qg_) {
   const __nv_bfloat16* q_nope = reinterpret_cast<const __nv_bfloat16*>(q_nope_v);
   const __nv_bfloat16* q_pe = reinterpret_cast<const __nv_bfloat16*>(q_pe_v);
   const __nv_bfloat16* kv = reinterpret_cast<const __nv_bfloat16*>(kv_v);
@@ -84,18 +96,24 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
   uint8_t* q_ring = smem + MLA_K_AREA;
   MlaBars* bars = reinterpret_cast<MlaBars*>(q_ring + MLA_Q_RING);
 
-  const int split = blockIdx.x, part = blockIdx.y, b = blockIdx.z;
+  const int Q = SPEC ? Q_ : 1, Qg = SPEC ? Qg_ : 1;
+  const int split = blockIdx.x, b = blockIdx.z;
+  const int part = SPEC ? blockIdx.y % MLA_PARTS : blockIdx.y, qg = SPEC ? blockIdx.y / MLA_PARTS : 0;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int S = seq_lens[b];
+  const int qn = SPEC ? min(Qg, Q - qg * Qg) : 1;   // draft tokens of this q-group
+  const int nrows = qn * Hq;                         // MMA rows that carry a query
+  const size_t row0 = (size_t)(b * Q + qg * Qg) * Hq;   // q / output row of MMA row 0
+  // keys of the group's last draft token: the most any row of this CTA sees (all of them when Q = 1)
+  const int S = SPEC ? seq_lens[b] - Q + qg * Qg + qn : seq_lens[b];
   const int t_first = split * tiles_per_cta * MLA_TOK;
   // this CTA walks n_tiles consecutive 128-token tiles of the request with an online softmax: O stays in registers,
   // partial (O, m, l) leave the CTA once
   const int n_tiles = min(tiles_per_cta, (S - t_first + MLA_TOK - 1) / MLA_TOK);
-  const size_t pbase = ((size_t)b * Hq) * num_splits;
+  const size_t pbase = row0 * num_splits;
 
   if (n_tiles <= 0) {
-    // empty split: publish (m = -inf, l = 0) so that the merge ignores it
-    if (part == 0 && tid < Hq) {
+    // empty split: publish (m = -inf, l = 0) for every row of the q-group so that the merge ignores it
+    if (part == 0 && tid < nrows) {
       part_ml[(pbase + (size_t)tid * num_splits + split) * 2] = -CUDART_INF_F;
       part_ml[(pbase + (size_t)tid * num_splits + split) * 2 + 1] = 0.f;
     }
@@ -109,6 +127,8 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
     mbar_init(&bars->o_full, 2);
     fence_barrier_init();
   }
+  // row r is draft token j = r / Hq of the group (rows past its last token take that token's limit)
+  if (SPEC && tid < 128) bars->row_off[tid] = (int8_t)(qn - 1 - min(tid / Hq, qn - 1));
   __syncthreads();
   // k-block order of a tile: the seven blocks the PV MMA of THIS CTA does not read (the other CTAs' value dims and the
   // rope block) come first — they can be refilled as soon as QK^T of the previous tile has completed, the two value
@@ -155,9 +175,9 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
             const int r = r0 + 16 * u;
             kreg[buf][u] = krow8[u] ? __ldg(reinterpret_cast<const uint2*>(krow8[u] + kb * 64 + c * 8)) : make_uint2(0u, 0u);
             qreg[buf][u] = make_uint2(0u, 0u);
-            if (q8 && r < Hq)
-              qreg[buf][u] = __ldg(reinterpret_cast<const uint2*>(kb < 8 ? qn8 + ((size_t)b * Hq + r) * 512 + kb * 64 + c * 8
-                                                                           : qp8 + ((size_t)b * Hq + r) * 64 + c * 8));
+            if (q8 && r < nrows)
+              qreg[buf][u] = __ldg(reinterpret_cast<const uint2*>(kb < 8 ? qn8 + (row0 + r) * 512 + kb * 64 + c * 8
+                                                                           : qp8 + (row0 + r) * 64 + c * 8));
           }
         };
 #pragma unroll
@@ -175,10 +195,10 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
             if (q8) {
               *reinterpret_cast<uint4*>(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(qreg[buf][u]);
             } else {
-              const bool qok = r < Hq;
+              const bool qok = r < nrows;
               const __nv_bfloat16* qsrc = !qok ? q_nope
-                                               : (kb < 8 ? q_nope + ((size_t)b * Hq + r) * 512 + kb * 64 + c * 8
-                                                         : q_pe + ((size_t)b * Hq + r) * 64 + c * 8);
+                                               : (kb < 8 ? q_nope + (row0 + r) * 512 + kb * 64 + c * 8
+                                                         : q_pe + (row0 + r) * 64 + c * 8);
               cp_async16(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16), qsrc, qok);
             }
             *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(kreg[buf][u]);
@@ -197,10 +217,10 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
             const int r = r0 + 16 * u;
-            const bool qok = r < Hq;
+            const bool qok = r < nrows;
             const __nv_bfloat16* qsrc = !qok ? q_nope
-                                             : (kb < 8 ? q_nope + ((size_t)b * Hq + r) * 512 + kb * 64 + c * 8
-                                                       : q_pe + ((size_t)b * Hq + r) * 64 + c * 8);
+                                             : (kb < 8 ? q_nope + (row0 + r) * 512 + kb * 64 + c * 8
+                                                       : q_pe + (row0 + r) * 64 + c * 8);
             cp_async16(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16), qsrc, qok);
             const bool kok = krow[u] != nullptr;
             cp_async16(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16), kok ? krow[u] + kb * 64 + c * 8 : kv, kok);
@@ -211,7 +231,7 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
     }
   } else {
     // ======================================================================= consumer warpgroups (64 heads each)
-    // accumulator fragment (wgmma.cuh): this thread holds heads h0 and h0 + 8, tokens / dims 8j + 2(lane % 4) and + 1
+    // accumulator fragment (wgmma.cuh): this thread holds rows h0 and h0 + 8, tokens / dims 8j + 2(lane % 4) and + 1
     const int wg = warp >> 2;
     const bool lead = (tid & 127) == 0;
     const int quad = lane & 3;
@@ -219,9 +239,17 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
     float sacc[MLA_TOK / 2], oacc[MLA_DV / 2];
     float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F};   // running row maxima (raw logits)
     float l[2] = {0.f, 0.f};                           // this thread's share of the row sums
+    // SPEC: row h0 + 8r sees the keys before S - row_off (its draft token j sees S - (qn - 1 - j) keys); its masked logits
+    // are set to -inf right after QK^T, so that no per-row limit stays live through the P loop (the consumers have no
+    // registers to spare; for the same reason the offsets are read from shared memory every tile).  The visible keys of a
+    // row are a prefix of the sequence, so a row that sees nothing in the CTA's first tile sees nothing in any later one:
+    // its m_run stays -inf (the lazy-rescale test compares NaN, which is false), it takes ms = 0 so that every P of it is
+    // exp2(-inf) = 0 (exp2f never sees -inf - -inf), and it publishes exactly m = -inf, l = 0, O = 0, which the merges skip.
     uint32_t qit = 0;
     for (int ti = 0; ti < n_tiles; ++ti) {
       const int nt = min(MLA_TOK, S - (t_first + ti * MLA_TOK));
+      // valid tokens of the tile per row (row h0 + 8r), t < ntr[r]
+      const int ntr[2] = {S - (t_first + ti * MLA_TOK) - bars->row_off[h0], S - (t_first + ti * MLA_TOK) - bars->row_off[h0 + 8]};
       // S = Q K^T over the nine k-blocks, in the order the loaders fill them
       for (int j = 0; j < MLA_KB; ++j, ++qit) {
         const int kb = kb_of(j);
@@ -240,12 +268,17 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
         if (lead) mbar_arrive(&bars->empty[s]);
       }
       if (lead) mbar_arrive(&bars->s_full);
+      if (SPEC) {   // masked logits -> -inf once, so that no per-row limit stays live through the P loop
+#pragma unroll
+        for (int i = 0; i < MLA_TOK / 2; ++i)
+          if ((i >> 2) * 8 + quad * 2 + (i & 1) >= ntr[(i >> 1) & 1]) sacc[i] = -CUDART_INF_F;
+      }
       // row maxima over the valid tokens of the tile: own columns, then the quad
       float m[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
       for (int i = 0; i < MLA_TOK / 2; ++i) {
         const int t = (i >> 2) * 8 + quad * 2 + (i & 1);
-        if (t < nt) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], sacc[i]);
+        if (SPEC || t < nt) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], sacc[i]);
       }
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
@@ -267,15 +300,17 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
             if (((i >> 1) & 1) == r) oacc[i] *= factor;
           l[r] *= factor;
         }
-        ms[r] = m_run[r] * scale_log2;
+        // SPEC: a row with no visible key so far (m_run = -inf) takes ms = 0, so that its masked logits give
+        // exp2(-inf - 0) = 0 and never -inf - -inf
+        ms[r] = SPEC && m_run[r] == -CUDART_INF_F ? 0.f : m_run[r] * scale_log2;
       }
       // P = exp2(s*scale - m*scale) -> bf16 pairs: the accumulator fragment of 16 tokens IS the A fragment of a k-step
       uint32_t pa[MLA_TOK / 16][4];
 #pragma unroll
       for (int i = 0; i < MLA_TOK / 2; i += 2) {
         const int t = (i >> 2) * 8 + quad * 2, r = (i >> 1) & 1;
-        const float p0 = (t < nt) ? exp2f(fmaf(sacc[i], scale_log2, -ms[r])) : 0.f;
-        const float p1 = (t + 1 < nt) ? exp2f(fmaf(sacc[i + 1], scale_log2, -ms[r])) : 0.f;
+        const float p0 = (SPEC || t < nt) ? exp2f(fmaf(sacc[i], scale_log2, -ms[r])) : 0.f;
+        const float p1 = (SPEC || t + 1 < nt) ? exp2f(fmaf(sacc[i + 1], scale_log2, -ms[r])) : 0.f;
         const __nv_bfloat162 pb = __floats2bfloat162_rn(p0, p1);
         // accumulate l from the ROUNDED probabilities so that O / l is consistent with the bf16 P used by the MMA
         l[r] += __low2float(pb) + __high2float(pb);
@@ -297,8 +332,8 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
     for (int r = 0; r < 2; ++r) {
       l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
       l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
-      const int h = h0 + 8 * r;
-      if (h < Hq) {
+      const int h = h0 + 8 * r;   // MMA row: q / output row row0 + h
+      if (h < nrows) {
         float* po = part_o + (pbase + (size_t)h * num_splits + split) * 512 + part * MLA_DV + quad * 2;
 #pragma unroll
         for (int j = 0; j < MLA_DV / 8; ++j)
@@ -313,13 +348,14 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
 }
 
 int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const void* kv, const int32_t* seq_lens,
-                  const int32_t* page_table, int batch, int Hq, int page_size, int max_pages, float sm_scale,
+                  const int32_t* page_table, int batch, int q_len, int Hq, int page_size, int max_pages, float sm_scale,
                   int num_splits, float* part_o, float* part_ml, int kv_fp8, int q_fp8, float descale_q, float descale_k) {
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(mla_decode_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MLA_SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(mla_decode_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MLA_SMEM);
+    cudaError_t e = cudaSuccess;
+    for (auto k : {mla_decode_tc_kernel<false, false>, mla_decode_tc_kernel<true, false>, mla_decode_tc_kernel<false, true>,
+                   mla_decode_tc_kernel<true, true>})
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, MLA_SMEM);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(mla_decode_tc)");
     attr = true;
   }
@@ -327,19 +363,20 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
     set_error("b200_mla_decode: e4m3 queries need the e4m3 cache");
     return B200_ERR_INVALID;
   }
-  dim3 grid(num_splits, MLA_PARTS, batch);
+  // draft tokens per q-group (as many as fill the 128 MMA rows), q-groups; the q-group varies with the part in grid.y
+  const int Qg = min(q_len, 128 / Hq), n_qg = (q_len + Qg - 1) / Qg;
+  dim3 grid(num_splits, MLA_PARTS * n_qg, batch);
   // each CTA walks tpc consecutive 128-token tiles (online softmax); the splits together cover the page table
   const int tiles = (int)(((int64_t)max_pages * page_size + MLA_TOK - 1) / MLA_TOK);
   const int tpc = (tiles + num_splits - 1) / num_splits;
   // descales (reference cutlass_mla.py: q_scale * k_scale folded into the softmax scale, k_scale into the output)
   const float sl2 = sm_scale * 1.4426950408889634f * (kv_fp8 ? descale_k * (q_fp8 ? descale_q : 1.f) : 1.f);
   const float osc = kv_fp8 ? descale_k : 1.f;
-  if (kv_fp8)
-    mla_decode_tc_kernel<true><<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size,
-                                                                   max_pages, sl2, num_splits, part_o, part_ml, q_fp8, osc, tpc);
-  else
-    mla_decode_tc_kernel<false><<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size,
-                                                                    max_pages, sl2, num_splits, part_o, part_ml, 0, 1.f, tpc);
+  const bool spec = q_len > 1;
+  auto kern = kv_fp8 ? (spec ? mla_decode_tc_kernel<true, true> : mla_decode_tc_kernel<true, false>)
+                     : (spec ? mla_decode_tc_kernel<false, true> : mla_decode_tc_kernel<false, false>);
+  kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size, max_pages, sl2, num_splits,
+                                            part_o, part_ml, kv_fp8 ? q_fp8 : 0, kv_fp8 ? osc : 1.f, tpc, q_len, Qg);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc launch");

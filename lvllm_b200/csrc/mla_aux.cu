@@ -101,9 +101,10 @@ __global__ void __launch_bounds__(128)
   }
 }
 
-// grid = B*Hq, 512 threads.  Partials from mla_decode_tc_kernel: part_o [B*Hq][splits][512] (un-normalised),
-// part_ml [B*Hq][splits][2] = (m * scale * log2e, l).  out_v [B,Hq,128] = (merged o, rounded to bf16 as the unfused
-// path would) x W_UV[h] ([512,128]); out_o (optional) the merged latent output [B,Hq,512]; lse optional.
+// grid = B*Q*Hq (rows w = (b * Q + i) * Hq + h), 512 threads.  Partials from mla_decode_tc_kernel: part_o [B*Q*Hq][splits][512]
+// (un-normalised), part_ml [B*Q*Hq][splits][2] = (m * scale * log2e, l).  out_v [B*Q,Hq,128] = (merged o, rounded to bf16 as
+// the unfused path would) x W_UV[h] ([512,128]); out_o (optional) the merged latent output [B*Q,Hq,512]; lse optional.  A row
+// whose every split published m = -inf (no visible key) gets out_v = 0, out_o = 0 and lse = -inf.
 __global__ void __launch_bounds__(512)
     mla_merge_vup_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml, int num_splits, int Hq,
                          const __nv_bfloat16* __restrict__ w_uv, __nv_bfloat16* __restrict__ out_v,
@@ -215,6 +216,13 @@ __global__ void __launch_bounds__(512)
   }
 }
 
+void launch_mla_merge_vup(cudaStream_t st, const float* part_o, const float* part_ml, int rows, int num_splits, int Hq,
+                          const void* w_uv, void* out_v, void* out_latent, float* lse) {
+  mla_merge_vup_kernel<<<rows * Hq, 512, 0, st>>>(part_o, part_ml, num_splits, Hq, reinterpret_cast<const __nv_bfloat16*>(w_uv),
+                                                 reinterpret_cast<__nv_bfloat16*>(out_v),
+                                                 reinterpret_cast<__nv_bfloat16*>(out_latent), lse);
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -259,25 +267,13 @@ int b200_mla_decode_vup(void* stream, const void* q_nope, const void* q_pe, int 
                         float descale_q, float descale_k, const int32_t* seq_lens, const int32_t* page_table, int batch,
                         int num_heads, int page_size, int max_pages, float sm_scale, int num_splits, void* workspace,
                         const void* w_uv, void* out_v, void* out_latent, float* lse) {
-  if (!q_nope || !q_pe || !kv_cache || !seq_lens || !page_table || !workspace || !w_uv || !out_v || batch <= 0 ||
-      num_heads <= 0 || num_heads > 128 || page_size <= 0 || num_splits <= 0 || num_splits > 512) {
-    set_error("b200_mla_decode_vup: bad argument (num_heads <= 128, num_splits <= 512)");
+  if (!w_uv) {   // without W_UV this is b200_mla_decode_ex, which has its own entry point
+    set_error("b200_mla_decode_vup: bad argument (w_uv, num_heads <= 128, num_splits <= 512)");
     return B200_ERR_INVALID;
   }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  float* po = reinterpret_cast<float*>(workspace);
-  float* pml = po + (size_t)batch * num_heads * num_splits * 512;
-  int rc = launch_mla_tc(st, q_nope, q_pe, kv_cache, seq_lens, page_table, batch, num_heads, page_size, max_pages, sm_scale,
-                         num_splits, po, pml, kv_dtype, q_dtype, descale_q, descale_k);
-  if (rc) return rc;
-  mla_merge_vup_kernel<<<batch * num_heads, 512, 0, st>>>(po, pml, num_splits, num_heads,
-                                                         reinterpret_cast<const __nv_bfloat16*>(w_uv),
-                                                         reinterpret_cast<__nv_bfloat16*>(out_v),
-                                                         reinterpret_cast<__nv_bfloat16*>(out_latent), lse);
-  ++g_launches;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "mla_merge_vup launch");
-  return 0;
+  return b200_mla_decode_spec(stream, q_nope, q_pe, q_dtype, kv_cache, kv_dtype, descale_q, descale_k, seq_lens, page_table,
+                              batch, 1, num_heads, page_size, max_pages, sm_scale, num_splits, workspace, out_latent, lse,
+                              w_uv, out_v);
 }
 
 }  // extern "C"

@@ -153,9 +153,12 @@ int repack_weights_w4(b200moe_layer* L, int e0, int ne, const void* w13_dev, con
                       const void* s2_dev, const void* g13_dev, const void* g2_dev, cudaStream_t st);
 int pick_tn_max(int M, int k, int E);
 int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const void* kv, const int32_t* seq_lens,
-                  const int32_t* page_table, int batch, int Hq, int page_size, int max_pages, float sm_scale,
+                  const int32_t* page_table, int batch, int q_len, int Hq, int page_size, int max_pages, float sm_scale,
                   int num_splits, float* part_o, float* part_ml, int kv_fp8 = 0, int q_fp8 = 0, float descale_q = 1.f,
                   float descale_k = 1.f);
+// split merge of the MLA partials fused with the v up-projection (mla_aux.cu), over rows (b * q_len + i, h)
+void launch_mla_merge_vup(cudaStream_t st, const float* part_o, const float* part_ml, int rows, int num_splits, int Hq,
+                          const void* w_uv, void* out_v, void* out_latent, float* lse);
 int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc, int64_t block_stride, int64_t page_stride,
                   int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table, int batch, int q_len, int Hq,
                   int Hkv, int page_size, int max_pages, float sm_scale, int num_splits, float* part_o, float* part_ml,

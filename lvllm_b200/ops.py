@@ -175,53 +175,63 @@ def rmsnorm_cast(x_f32: torch.Tensor, out: torch.Tensor, gain: float = 1.0, eps:
 
 def mla_decode(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_c_and_k_pe_cache: torch.Tensor, seq_lens: torch.Tensor,
                page_table: torch.Tensor, sm_scale: float, num_kv_splits: int = 0, max_seq_len: int | None = None,
-               q_scale: float = 1.0, k_scale: float = 1.0, w_uv: torch.Tensor | None = None):
+               q_scale: float = 1.0, k_scale: float = 1.0, w_uv: torch.Tensor | None = None, q_len_per_req: int = 1):
     """Paged MLA decode; mirrors ops.sm100_cutlass_mla_decode (reference vllm/_custom_ops.py:3212,
     backends/mla/cutlass_mla.py:176-257).  bf16 q + bf16 cache, or an e4m3 cache (``torch.float8_e4m3fn``, 576 B / token)
     with bf16 or e4m3 queries (the reference's fp8 mode; q_scale / k_scale = per-tensor dequantisation scales).
     ``max_seq_len`` (host-side bound on seq_lens) sizes the split count / workspace instead of the page-table width.
-    With ``w_uv`` [Hq,512,128] the split merge is fused with the v up-projection and (out_v [B,Hq,128], out, lse) is returned.
-    Returns (out bf16 [B,Hq,512], lse f32 [B,Hq])."""
+    B = seq_lens.numel(); Q = ``q_len_per_req`` query tokens per request (speculative-decode verification of
+    multi-token-prediction drafts, the reference FlashMLA backend's uniform query length with causal=True,
+    backends/mla/flashmla.py:120, :284-344): q_nope [B*Q,Hq,512] / q_pe [B*Q,Hq,64] hold request b's Q tokens contiguous in
+    draft order, seq_lens[b] counts all its keys including the Q new ones, and token i attends to keys
+    [0, seq_lens[b] - Q + i] (a row with no visible key gives out 0 and lse -inf).  Q = 1 (the default) is the
+    single-token decode.
+    With ``w_uv`` [Hq,512,128] the split merge is fused with the v up-projection and (out_v [B*Q,Hq,128], out, lse) is
+    returned.  Returns (out bf16 [B*Q,Hq,512], lse f32 [B*Q,Hq])."""
     qn, qp = _cuda(q_nope, "q_nope"), _cuda(q_pe, "q_pe")
     kv = _cuda(kv_c_and_k_pe_cache, "kv_cache")
     f8 = torch.float8_e4m3fn
     assert kv.dtype in (torch.bfloat16, f8) and kv.shape[-1] == 576
     assert qn.dtype == qp.dtype and qn.dtype in (torch.bfloat16, f8) and (qn.dtype != f8 or kv.dtype == f8)
-    B, Hq, _ = qn.shape
+    T, Hq, _ = qn.shape
+    Q = int(q_len_per_req)
     page = kv.shape[1]
-    sl = _cuda(seq_lens.to(torch.int32), "seq_lens")
+    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
     pt = _cuda(page_table.to(torch.int32), "page_table")
+    B = sl.numel()
+    if T != B * Q or qp.shape[0] != T:
+        raise ValueError(f"q_nope / q_pe must hold q_len_per_req = {Q} tokens per request: {B * Q} rows for {B} seq_lens, "
+                         f"got {T} / {qp.shape[0]}")
+    if pt.dim() != 2 or pt.shape[0] < B:   # the kernel reads row b of the table for every request b < B
+        raise ValueError(f"page_table must have a row per request ({B}), got {tuple(pt.shape)}")
     max_pages = pt.shape[1]
     if max_seq_len is not None:
         # the kernel only walks pages below the bound: a narrower view of the table keeps the split count (and the
-        # B*Hq*splits*514*4-byte workspace) proportional to the real context, not to max_model_len
+        # B*Q*Hq*splits*514*4-byte workspace) proportional to the real context, not to max_model_len
         max_pages = min(max_pages, -(-int(max_seq_len) // page))
         if max_pages != pt.shape[1]:
             pt = pt[:, :max_pages].contiguous()
     if num_kv_splits <= 0:
-        # a CTA = (request, split, value-dim quarter) walks ceil(tiles / splits) 128-token tiles with an online softmax:
-        # enough splits to fill ~2 waves of the 132 SMs, no more (each split costs an fp32 partial of the output)
+        # a CTA = (request, q-group, split, value-dim quarter) walks ceil(tiles / splits) 128-token tiles with an online
+        # softmax: enough splits to fill ~2 waves of the 132 SMs, no more (each split costs an fp32 partial of the output)
         tiles = max(1, -(-(max_pages * page) // 128))
-        num_kv_splits = max(1, min(tiles, 264 // (4 * B)))
-    ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(B, Hq, num_kv_splits), dtype=torch.uint8, device=qn.device)
-    out = torch.empty(B, Hq, 512, dtype=torch.bfloat16, device=qn.device)
-    lse = torch.empty(B, Hq, dtype=torch.float32, device=qn.device)
+        qg = max(1, min(Q, 128 // Hq))   # draft tokens per q-group (the kernel's 128 MMA rows); n_qg q-groups
+        n_qg = -(-Q // qg)
+        num_kv_splits = max(1, min(tiles, 264 // (4 * B * n_qg)))
+    ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(T, Hq, num_kv_splits), dtype=torch.uint8, device=qn.device)
+    out = torch.empty(T, Hq, 512, dtype=torch.bfloat16, device=qn.device)
+    lse = torch.empty(T, Hq, dtype=torch.float32, device=qn.device)
+    args = [_stream(), qn.data_ptr(), qp.data_ptr(), int(qn.dtype == f8), kv.data_ptr(), int(kv.dtype == f8), float(q_scale),
+            float(k_scale), sl.data_ptr(), pt.data_ptr(), B, Q, Hq, page, max_pages, float(sm_scale), num_kv_splits,
+            ws.data_ptr(), out.data_ptr(), lse.data_ptr()]
     if w_uv is not None:
         # split merge fused with the v up-projection (reference _v_up_proj, mla_attention.py:1154-1176)
         wv = _cuda(w_uv, "w_uv")
         assert wv.dtype == torch.bfloat16 and wv.shape == (Hq, 512, 128)
-        out_v = torch.empty(B, Hq, 128, dtype=torch.bfloat16, device=qn.device)
-        rc = L.lib().b200_mla_decode_vup(_stream(), qn.data_ptr(), qp.data_ptr(), int(qn.dtype == f8), kv.data_ptr(),
-                                         int(kv.dtype == f8), float(q_scale), float(k_scale), sl.data_ptr(), pt.data_ptr(),
-                                         B, Hq, page, max_pages, float(sm_scale), num_kv_splits, ws.data_ptr(),
-                                         wv.data_ptr(), out_v.data_ptr(), out.data_ptr(), lse.data_ptr())
-        L.check(rc, "b200_mla_decode_vup")
+        out_v = torch.empty(T, Hq, 128, dtype=torch.bfloat16, device=qn.device)
+        L.check(L.lib().b200_mla_decode_spec(*args, wv.data_ptr(), out_v.data_ptr()), "b200_mla_decode_vup")
         return out_v, out, lse
-    rc = L.lib().b200_mla_decode_ex(_stream(), qn.data_ptr(), qp.data_ptr(), int(qn.dtype == f8), kv.data_ptr(),
-                                    int(kv.dtype == f8), float(q_scale), float(k_scale), sl.data_ptr(), pt.data_ptr(),
-                                    B, Hq, page, max_pages, float(sm_scale), num_kv_splits, ws.data_ptr(),
-                                    out.data_ptr(), lse.data_ptr())
-    L.check(rc, "b200_mla_decode")
+    L.check(L.lib().b200_mla_decode_spec(*args, None, None), "b200_mla_decode")
     return out, lse
 
 
