@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -104,10 +105,59 @@ int tm_encode_2d(CUtensorMap* tm, int dtype, const void* base, uint64_t d0, uint
   return 0;
 }
 
+// Per-device launch set-up.  A kernel's dynamic shared-memory limit is an attribute of the device's context, so it is
+// raised once per (device, kernel); the SM counts and cpu_prefill's streams are per device too.
+static std::mutex g_setup_mu;
+static std::map<std::pair<int, const void*>, int> g_smem_set;
+static std::map<int, int> g_sms;
+static std::map<int, cudaStream_t> g_prefill_stream;
+
+int kernel_smem(const void* fn, int bytes, const char* what) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
+  std::lock_guard<std::mutex> lk(g_setup_mu);
+  int& set = g_smem_set[{dev, fn}];
+  if (bytes <= set) return 0;
+  e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return cuda_fail(e, what);
+  set = bytes;
+  return 0;
+}
+
+int device_sms(int dev) {
+  std::lock_guard<std::mutex> lk(g_setup_mu);
+  int& n = g_sms[dev];
+  if (!n) {
+    cudaError_t e = cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) {
+      n = 0;
+      return cuda_fail(e, "cudaDeviceGetAttribute(SM count)");
+    }
+  }
+  return n;
+}
+
 static bool stream_capturing(cudaStream_t st) {
   cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
   if (cudaStreamIsCapturing(st, &s) != cudaSuccess) return false;
   return s != cudaStreamCaptureStatusNone;
+}
+
+// All layers and streams of a device share one workspace and the fused kernel's cross-CTA counters.  Calls on one
+// stream are ordered by the stream; an eager call arriving on ANOTHER stream is ordered behind the previous one with
+// an event (graph-captured calls are ordered by the graph's own edges: Lvllm captures one stream).
+static void wait_last_use(Workspace* ws, cudaStream_t st) {
+  std::lock_guard<std::mutex> lk(g_prof_mu);
+  if (ws->last_valid && ws->last_stream != st) cudaStreamWaitEvent(st, ws->last_use, 0);
+}
+
+static void record_last_use(Workspace* ws, cudaStream_t st) {
+  std::lock_guard<std::mutex> lk(g_prof_mu);
+  if (!ws->last_use) cudaEventCreateWithFlags(&ws->last_use, cudaEventDisableTiming);
+  cudaEventRecord(ws->last_use, st);
+  ws->last_stream = st;
+  ws->last_valid = true;
 }
 
 // one full forward of the routed experts on device buffers
@@ -120,13 +170,7 @@ static int forward_device(b200moe_layer* L, cudaStream_t st, int M, int k, const
   }
   Workspace* ws = get_workspace(L->device);
   const bool cap = stream_capturing(st);
-  // All layers and streams of a device share one workspace and the fused kernel's cross-CTA counters.  Calls on one
-  // stream are ordered by the stream; an eager call arriving on ANOTHER stream is ordered behind the previous one
-  // with an event (graph-captured calls are ordered by the graph's own edges: Lvllm captures one stream).
-  if (!cap) {
-    std::lock_guard<std::mutex> lk(g_prof_mu);
-    if (ws->last_valid && ws->last_stream != st) cudaStreamWaitEvent(st, ws->last_use, 0);
-  }
+  if (!cap) wait_last_use(ws, st);
   // 4-bit layers, prefill-class batches (eager calls only): expand the experts once into fp16 tiles and run the batch
   // through the 16-bit grouped GEMM in passes of up to 8192 tokens, instead of re-streaming the packed weights through
   // the fused decode kernel once per 256 tokens.  W4A16 numerics for every 4-bit format on this path (native-MX layers
@@ -135,8 +179,12 @@ static int forward_device(b200moe_layer* L, cudaStream_t st, int M, int k, const
     const char* v = getenv("B200MOE_W4_PREFILL_MIN");
     return v ? atoi(v) : 1024;
   }();
-  if (L->wq && !cap && w4_prefill_min > 0 && M >= w4_prefill_min) {
-    b200moe_layer P = *L;   // fp16 shadow of the layer: same geometry, expanded weights
+  const bool expand = L->wq && !cap && w4_prefill_min > 0 && M >= w4_prefill_min;
+  b200moe_layer P;                 // fp16 shadow of a 4-bit layer: same geometry, expanded weights
+  const b200moe_layer* V = L;      // the layer the passes run
+  int pass;
+  if (expand) {
+    P = *L;
     P.wq = 0;
     P.esz_bits = 16;
     P.KB1 = L->H / 64;
@@ -150,76 +198,55 @@ static int forward_device(b200moe_layer* L, cudaStream_t st, int M, int k, const
     P.w13t = ws->dq13;
     P.w2t = ws->dq2;
     if ((rc = launch_w4_dequant(L, ws->dq13, ws->dq2, st))) return rc;
-    int pp = L->cfg.max_batch_size > 0 ? L->cfg.max_batch_size : 4096;
-    if (pp > 8192) pp = 8192;
-    if (pp < 256) pp = 256;
-    for (int t0 = 0; t0 < M; t0 += pp) {
-      const int m = (M - t0 < pp) ? (M - t0) : pp;
-      if ((rc = ensure_workspace(ws, &P, m, k, true))) return rc;
-      const size_t osz = (out_dtype == 2) ? 4 : 2;
-      void* optr = reinterpret_cast<uint8_t*>(out) + (size_t)t0 * L->H * osz;
-      const int tn_max = pick_tn_max(m, k, L->E);
-      const uint8_t* hptr = reinterpret_cast<const uint8_t*>(hidden) + (size_t)t0 * L->H * 2;
-      if ((rc = launch_prep(&P, ws, st, hptr, ids + (size_t)t0 * k, m, k, tn_max))) return rc;
-      cudaEvent_t* ev = g_profile ? next_events(false) : nullptr;
-      if ((rc = launch_gemms(&P, ws, st, m, k, tn_max, ev))) return rc;
-      if ((rc = launch_combine(&P, ws, st, w + (size_t)t0 * k, m, k, optr, out_dtype))) return rc;
-    }
-    std::lock_guard<std::mutex> lk(g_prof_mu);
-    if (!ws->last_use) cudaEventCreateWithFlags(&ws->last_use, cudaEventDisableTiming);
-    cudaEventRecord(ws->last_use, st);
-    ws->last_stream = st;
-    ws->last_valid = true;
-    return 0;
-  }
-  // passes bound the workspace for very large prefill batches; below the prefill threshold 4-bit formats run through
-  // the fused decode kernel, so their pass is the largest batch that kernel's tables hold (M * top_k <= 2048 slots)
-  int pass = L->max_tokens;
-  if (L->wq) {
-    if (pass > FUSED_MAX_TOKENS) pass = FUSED_MAX_TOKENS;
-    while (pass > 1 && !fused_supported(L, pass, k)) pass = pass > 16 ? pass - 8 : pass - 1;
-    if (!fused_supported(L, pass, k)) {
-      set_error("4-bit formats are served by the fused decode kernel only and this layer / top_k is outside its limits "
-                "(experts <= 512, top_k <= 2048 slots per pass)");
-      return B200_ERR_INVALID;
+    V = &P;
+    pass = L->cfg.max_batch_size > 0 ? L->cfg.max_batch_size : 4096;
+    if (pass > 8192) pass = 8192;
+    if (pass < 256) pass = 256;
+  } else {
+    // passes bound the workspace for very large prefill batches; below the prefill threshold 4-bit formats run through
+    // the fused decode kernel, so their pass is the largest batch that kernel's tables hold (M * top_k <= 2048 slots)
+    pass = L->max_tokens;
+    if (L->wq) {
+      if (pass > FUSED_MAX_TOKENS) pass = FUSED_MAX_TOKENS;
+      while (pass > 1 && !fused_supported(L, pass, k)) pass = pass > 16 ? pass - 8 : pass - 1;
+      if (!fused_supported(L, pass, k)) {
+        set_error("4-bit formats are served by the fused decode kernel only and this layer / top_k is outside its limits "
+                  "(experts <= 512, top_k <= 2048 slots per pass)");
+        return B200_ERR_INVALID;
+      }
     }
   }
   for (int t0 = 0; t0 < M; t0 += pass) {
     const int m = (M - t0 < pass) ? (M - t0) : pass;
-    int rc = ensure_workspace(ws, L, m, k, !cap);
+    int rc = ensure_workspace(ws, V, m, k, !cap);
     if (rc) return rc;
     const size_t osz = (out_dtype == 2) ? 4 : 2;
     void* optr = reinterpret_cast<uint8_t*>(out) + (size_t)t0 * L->H * osz;
-    if (fused_supported(L, m, k)) {
+    const uint8_t* hptr = reinterpret_cast<const uint8_t*>(hidden) + (size_t)t0 * L->H * 2;
+    // The fp16 shadow never takes the fused kernel: launch_fused ignores cvt_bf16_to_fp16 (it would read bf16 rows as
+    // fp16), and with fp16 activations a short last pass would switch kernels and so change bits.
+    if (!expand && fused_supported(L, m, k)) {
       cudaEvent_t* fev = nullptr;
       if (g_profile && !cap) {
         fev = next_events(true);
         cudaEventRecord(fev[0], st);
       }
-      rc = launch_fused(L, ws, st, reinterpret_cast<const uint8_t*>(hidden) + (size_t)t0 * L->H * 2,
-                        ids + (size_t)t0 * k, w + (size_t)t0 * k, m, k, optr, out_dtype);
+      rc = launch_fused(L, ws, st, hptr, ids + (size_t)t0 * k, w + (size_t)t0 * k, m, k, optr, out_dtype);
       if (fev) cudaEventRecord(fev[1], st);
       if (rc) return rc;
       continue;
     }
-    if (L->wq) {
+    if (V->wq) {
       set_error("4-bit formats are served by the fused decode kernel only (this call is outside its limits)");
       return B200_ERR_INVALID;
     }
     const int tn_max = pick_tn_max(m, k, L->E);
-    const uint8_t* hptr = reinterpret_cast<const uint8_t*>(hidden) + (size_t)t0 * L->H * 2;
-    if ((rc = launch_prep(L, ws, st, hptr, ids + (size_t)t0 * k, m, k, tn_max))) return rc;
+    if ((rc = launch_prep(V, ws, st, hptr, ids + (size_t)t0 * k, m, k, tn_max))) return rc;
     cudaEvent_t* ev = (g_profile && !cap) ? next_events(false) : nullptr;
-    if ((rc = launch_gemms(L, ws, st, m, k, tn_max, ev))) return rc;
-    if ((rc = launch_combine(L, ws, st, w + (size_t)t0 * k, m, k, optr, out_dtype))) return rc;
+    if ((rc = launch_gemms(V, ws, st, m, k, tn_max, ev))) return rc;
+    if ((rc = launch_combine(V, ws, st, w + (size_t)t0 * k, m, k, optr, out_dtype))) return rc;
   }
-  if (!cap) {
-    std::lock_guard<std::mutex> lk(g_prof_mu);
-    if (!ws->last_use) cudaEventCreateWithFlags(&ws->last_use, cudaEventDisableTiming);
-    cudaEventRecord(ws->last_use, st);
-    ws->last_stream = st;
-    ws->last_valid = true;
-  }
+  if (!cap) record_last_use(ws, st);
   return 0;
 }
 
@@ -233,16 +260,11 @@ const char* b200moe_last_error(void) { return g_err.c_str(); }
 const char* b200moe_version(void) { return "b200moe 0.1 sm_90a"; }
 int64_t b200moe_launch_count(void) { return g_launches; }
 
-// validation + layer geometry shared by b200moe_create and b200moe_create_empty (`have_*`: which tensors the format needs
-// is checked against what the caller says it will provide)
-static int make_layer(const b200moe_config* cfg, bool have_scales, bool have_gscales, int format, int act_dtype,
-                      b200moe_layer** out_layer) {
-  const void* w13_scale = have_scales ? cfg : nullptr;          // only tested for null-ness below
-  const void* w2_scale = w13_scale;
-  const void* w13_global_scale = have_gscales ? cfg : nullptr;
-  const void* w2_global_scale = w13_global_scale;
-  if (!cfg || !out_layer) {
-    set_error("b200moe_create: null config");
+// ---- per-expert ingest (SURVEY.md 8f row 4: checkpoint -> HBM without a stacked [E, ...] host tensor).  Validation
+// and layer geometry; which scale tensors the format needs is checked by b200moe_load_experts.
+int b200moe_create_empty(const b200moe_config* cfg, int format, int act_dtype, b200moe_handle* out) {
+  if (!cfg || !out) {
+    set_error("b200moe_create: null config / output");
     return B200_ERR_INVALID;
   }
   int dev = 0;
@@ -267,14 +289,6 @@ static int make_layer(const b200moe_config* cfg, bool have_scales, bool have_gsc
   }
   const bool w4 = (format == B200_FMT_WNA16 || format == B200_FMT_NVFP4 || format == B200_FMT_MXFP4);
   if (w4) {
-    if (!w13_scale || !w2_scale) {
-      set_error("b200moe_create: 4-bit formats need weight scales");
-      return B200_ERR_INVALID;
-    }
-    if (format == B200_FMT_NVFP4 && (!w13_global_scale || !w2_global_scale)) {
-      set_error("b200moe_create: NVFP4 needs the per-expert global scales");
-      return B200_ERR_INVALID;
-    }
     if (!cfg->has_gate_proj || (H / 128) % 2) {
       set_error("b200moe_create: 4-bit formats need gated experts and hidden_size % 256 == 0");
       return B200_ERR_INVALID;
@@ -286,10 +300,6 @@ static int make_layer(const b200moe_config* cfg, bool have_scales, bool have_gsc
       set_error("b200moe_create: unsupported 4-bit group shape (WNA16: groupK multiple of 32, NVFP4: 16, MXFP4: 32; groupN 1)");
       return B200_ERR_INVALID;
     }
-  }
-  if (format == B200_FMT_FP8 && (!w13_scale || !w2_scale)) {
-    set_error("b200moe_create: FP8 needs weight scales");
-    return B200_ERR_INVALID;
   }
   if (w4 && E > FUSED_MAX_EXPERTS) {
     set_error("b200moe_create: 4-bit formats support at most " + std::to_string(FUSED_MAX_EXPERTS) +
@@ -378,7 +388,7 @@ static int make_layer(const b200moe_config* cfg, bool have_scales, bool have_gsc
   if (mt > 8192) mt = 8192;
   if (w4 && mt > 256) mt = 256;   // 4-bit formats run through the fused decode kernel only: larger batches in passes
   L->max_tokens = mt;
-  *out_layer = L;
+  *out = L;
   return 0;
 }
 
@@ -467,51 +477,23 @@ static int ingest_range(b200moe_layer* L, int e0, int ne, const void* w13, const
   return rc;
 }
 
-static int finalize_layer(b200moe_layer* L) {
-  int rc;
-  // decode workspaces are allocated up front so that cpu_decode can run under stream capture
-  Workspace* ws = get_workspace(L->device);
-  if ((rc = ensure_workspace(ws, L, L->max_tokens, L->cfg.top_k, true))) return rc;
-  {
-    std::lock_guard<std::mutex> lk(g_prof_mu);
-    ++ws->live_layers;
-    L->counted = 1;
-  }
-  L->finalized = 1;
-  return 0;
-}
-
 int b200moe_create(const b200moe_config* cfg, const void* w13, const void* w2, const void* w13_scale,
                    const void* w2_scale, const void* w13_global_scale, const void* w2_global_scale, int format,
                    int act_dtype, int weights_on_device, b200moe_handle* out) {
-  if (!cfg || !out || !w13 || !w2) {
-    set_error("b200moe_create: null config / weight pointer");
+  if (!out) {
+    set_error("b200moe_create: null output");
     return B200_ERR_INVALID;
   }
-  b200moe_layer* L = nullptr;
-  int rc = make_layer(cfg, w13_scale && w2_scale, w13_global_scale && w2_global_scale, format, act_dtype, &L);
+  b200moe_handle L = nullptr;
+  int rc = b200moe_create_empty(cfg, format, act_dtype, &L);
   if (rc) return rc;
-  rc = ingest_range(L, 0, L->E, w13, w2, w13_scale, w2_scale, w13_global_scale, w2_global_scale, weights_on_device);
-  if (!rc) rc = finalize_layer(L);
+  rc = b200moe_load_experts(L, 0, L->E, w13, w2, w13_scale, w2_scale, w13_global_scale, w2_global_scale,
+                            weights_on_device);
+  if (!rc) rc = b200moe_finalize(L);
   if (rc) {
     b200moe_destroy(L);
     return rc;
   }
-  L->experts_loaded = L->E;
-  *out = L;
-  return 0;
-}
-
-// ---- per-expert ingest (SURVEY.md 8f row 4: checkpoint -> HBM without a stacked [E, ...] host tensor) -------------------
-int b200moe_create_empty(const b200moe_config* cfg, int format, int act_dtype, b200moe_handle* out) {
-  if (!out) {
-    set_error("b200moe_create_empty: null output");
-    return B200_ERR_INVALID;
-  }
-  b200moe_layer* L = nullptr;
-  const bool need_scales = format != B200_FMT_16BIT;
-  int rc = make_layer(cfg, need_scales, format == B200_FMT_NVFP4, format, act_dtype, &L);
-  if (rc) return rc;
   *out = L;
   return 0;
 }
@@ -542,7 +524,17 @@ int b200moe_finalize(b200moe_handle h) {
     set_error("b200moe_finalize: only " + std::to_string(h->experts_loaded) + " of " + std::to_string(h->E) + " experts were loaded");
     return B200_ERR_INVALID;
   }
-  return finalize_layer(h);
+  // decode workspaces are allocated up front so that cpu_decode can run under stream capture
+  Workspace* ws = get_workspace(h->device);
+  int rc = ensure_workspace(ws, h, h->max_tokens, h->cfg.top_k, true);
+  if (rc) return rc;
+  {
+    std::lock_guard<std::mutex> lk(g_prof_mu);
+    ++ws->live_layers;
+    h->counted = 1;
+  }
+  h->finalized = 1;
+  return 0;
 }
 
 int b200moe_destroy(b200moe_handle h) {
@@ -615,14 +607,15 @@ int b200moe_cpu_prefill(b200moe_handle h, int num_tokens, int top_k, const int32
   if (rc) return rc;
   // the caller has synchronised its stream (reference routed_experts.py:1866); the copies and kernels run on the
   // library's own non-blocking stream, ordered against eager calls of other streams by forward_device
-  static cudaStream_t pst[16] = {};
-  if (!pst[h->device] && (e = cudaStreamCreateWithFlags(&pst[h->device], cudaStreamNonBlocking)) != cudaSuccess)
-    return cuda_fail(e, "cudaStreamCreate(cpu_prefill)");
-  cudaStream_t st = pst[h->device];
+  cudaStream_t st = nullptr;
   {
-    std::lock_guard<std::mutex> lk(g_prof_mu);
-    if (ws->last_valid && ws->last_stream != st) cudaStreamWaitEvent(st, ws->last_use, 0);   // staging buffers are shared too
+    std::lock_guard<std::mutex> lk(g_setup_mu);
+    cudaStream_t& pst = g_prefill_stream[h->device];
+    if (!pst && (e = cudaStreamCreateWithFlags(&pst, cudaStreamNonBlocking)) != cudaSuccess)
+      return cuda_fail(e, "cudaStreamCreate(cpu_prefill)");
+    st = pst;
   }
+  wait_last_use(ws, st);   // staging buffers are shared too
   if ((e = cudaMemcpyAsync(ws->d_hidden, hidden_host, M * H * 2, cudaMemcpyHostToDevice, st)) != cudaSuccess) return cuda_fail(e, "H2D hidden");
   if ((e = cudaMemcpyAsync(ws->d_ids, ids_host, M * top_k * 4, cudaMemcpyHostToDevice, st)) != cudaSuccess) return cuda_fail(e, "H2D ids");
   if ((e = cudaMemcpyAsync(ws->d_w, w_host, M * top_k * 4, cudaMemcpyHostToDevice, st)) != cudaSuccess) return cuda_fail(e, "H2D weights");

@@ -413,19 +413,6 @@ int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc
                   int64_t head_stride, const int32_t* seq_lens, const int32_t* page_table, int batch, int q_len, int Hq,
                   int Hkv, int page_size, int max_pages, float sm_scale, int num_splits, float* part_o, float* part_ml,
                   void* out, float* lse) {
-  static bool attr = false;
-  static int num_sms = 0;
-  if (!attr) {
-    cudaError_t e = cudaSuccess;
-    for (auto k : {gqa_decode_tc_kernel<16, false>, gqa_decode_tc_kernel<32, false>, gqa_decode_tc_kernel<16, true>,
-                   gqa_decode_tc_kernel<32, true>})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, GQA_SMEM_MAX);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(gqa_decode_tc)");
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    attr = true;
-  }
   const int G = Hq / Hkv;
   if (G > GQA_MAX_N) return 1;   // not handled here
   const int Qg = min(q_len, GQA_MAX_N / G), n_qg = (q_len + Qg - 1) / Qg;   // draft tokens per q-group, q-groups
@@ -445,11 +432,17 @@ int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc
     return B200_ERR_INVALID;
   }
   const int smem = fixed + nst * stage_bytes;
+  int dev = 0;
+  if (const cudaError_t e = cudaGetDevice(&dev); e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
+  const int num_sms = device_sms(dev);
+  if (num_sms < 0) return num_sms;
   const int total = batch * Hkv * n_qg * num_splits;
   const int grid = total < num_sms ? total : num_sms;
   if ((total + grid - 1) / grid > GQA_MAX_ITEMS) return 1;   // not handled here: caller uses the split-KV CUDA-core path
-  auto kern = q_len > 1 ? (N == 16 ? gqa_decode_tc_kernel<16, true> : gqa_decode_tc_kernel<32, true>)
-                        : (N == 16 ? gqa_decode_tc_kernel<16, false> : gqa_decode_tc_kernel<32, false>);
+  auto kern = q_len == 1 ? (N == 16 ? gqa_decode_tc_kernel<16, false> : gqa_decode_tc_kernel<32, false>)
+                         : (N == 16 ? gqa_decode_tc_kernel<16, true> : gqa_decode_tc_kernel<32, true>);
+  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), GQA_SMEM_MAX, "cudaFuncSetAttribute(gqa_decode_tc)");
+  if (rc) return rc;
   kern<<<grid, GQA_THREADS, smem, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(kc),
       reinterpret_cast<const __nv_bfloat16*>(vc), seq_lens, block_stride, page_stride, head_stride, page_table, batch, Hq, Hkv, page_size, max_pages,

@@ -350,15 +350,6 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
 int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const void* kv, const int32_t* seq_lens,
                   const int32_t* page_table, int batch, int q_len, int Hq, int page_size, int max_pages, float sm_scale,
                   int num_splits, float* part_o, float* part_ml, int kv_fp8, int q_fp8, float descale_q, float descale_k) {
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaSuccess;
-    for (auto k : {mla_decode_tc_kernel<false, false>, mla_decode_tc_kernel<true, false>, mla_decode_tc_kernel<false, true>,
-                   mla_decode_tc_kernel<true, true>})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, MLA_SMEM);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(mla_decode_tc)");
-    attr = true;
-  }
   if (q_fp8 && !kv_fp8) {
     set_error("b200_mla_decode: e4m3 queries need the e4m3 cache");
     return B200_ERR_INVALID;
@@ -372,9 +363,10 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
   // descales (reference cutlass_mla.py: q_scale * k_scale folded into the softmax scale, k_scale into the output)
   const float sl2 = sm_scale * 1.4426950408889634f * (kv_fp8 ? descale_k * (q_fp8 ? descale_q : 1.f) : 1.f);
   const float osc = kv_fp8 ? descale_k : 1.f;
-  const bool spec = q_len > 1;
-  auto kern = kv_fp8 ? (spec ? mla_decode_tc_kernel<true, true> : mla_decode_tc_kernel<true, false>)
-                     : (spec ? mla_decode_tc_kernel<false, true> : mla_decode_tc_kernel<false, false>);
+  auto kern = q_len == 1 ? (!kv_fp8 ? mla_decode_tc_kernel<false, false> : mla_decode_tc_kernel<true, false>)
+                         : (!kv_fp8 ? mla_decode_tc_kernel<false, true> : mla_decode_tc_kernel<true, true>);
+  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc)");
+  if (rc) return rc;
   kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size, max_pages, sl2, num_splits,
                                             part_o, part_ml, kv_fp8 ? q_fp8 : 0, kv_fp8 ? osc : 1.f, tpc, q_len, Qg);
   ++g_launches;

@@ -1374,12 +1374,8 @@ template <bool FP8, int NA, int TNMAX, int WQ>
 static int launch_fused_t(const FusedArgs& a, cudaStream_t st, int num_sms) {
   using C = FCfg<FP8, NA, TNMAX, WQ>;
   auto kern = moe_fused_kernel<FP8, NA, TNMAX, WQ>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(moe_fused)");
-    attr_set = true;
-  }
+  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), C::SMEM, "cudaFuncSetAttribute(moe_fused)");
+  if (rc) return rc;
   // Cooperative launch: the cross-CTA spin waits need every CTA of the grid resident at once; a plain launch that
   // shares the GPU with another stream's kernels could be scheduled piecemeal and dead-lock.
   cudaLaunchConfig_t cfg{};
@@ -1415,13 +1411,8 @@ bool fused_supported(const b200moe_layer* L, int M, int k) {
 
 int launch_fused(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const void* hidden, const int32_t* ids,
                  const float* topk_w, int M, int k, void* out, int out_dtype) {
-  static int num_sms = 0;
-  if (!num_sms) {
-    cudaDeviceProp p;
-    cudaError_t e = cudaGetDeviceProperties(&p, L->device);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaGetDeviceProperties");
-    num_sms = p.multiProcessorCount;
-  }
+  const int num_sms = device_sms(L->device);
+  if (num_sms < 0) return num_sms;
   FusedArgs a{};
   a.w13t = L->w13t;
   a.w2t = L->w2t;

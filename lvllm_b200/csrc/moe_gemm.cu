@@ -427,12 +427,8 @@ template <int MODE, int NA, int EPI, int TNMAX>
 static int launch_one(const GemmArgs& a, cudaStream_t st, int num_sms) {
   using C = Cfg<MODE, NA, TNMAX>;
   auto kern = moe_gemm_kernel<MODE, NA, EPI, TNMAX>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(moe_gemm)");
-    attr_set = true;
-  }
+  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), C::SMEM, "cudaFuncSetAttribute(moe_gemm)");
+  if (rc) return rc;
   kern<<<num_sms, GEMM_THREADS, C::SMEM, st>>>(a);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
@@ -509,13 +505,8 @@ int pick_tn_max(int M, int k, int E) {
 }
 
 int launch_gemms(const b200moe_layer* L, Workspace* ws, cudaStream_t st, int M, int k, int tn_max, cudaEvent_t* ev) {
-  static int num_sms = 0;
-  if (!num_sms) {
-    cudaDeviceProp p;
-    cudaError_t e = cudaGetDeviceProperties(&p, L->device);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaGetDeviceProperties");
-    num_sms = p.multiProcessorCount;
-  }
+  const int num_sms = device_sms(L->device);
+  if (num_sms < 0) return num_sms;
   const bool fp8 = (L->esz_bits == 8);
   switch (tn_max) {
     case 16: return fp8 ? launch_pair<MODE_FP8, 16>(L, ws, st, num_sms, ev) : launch_pair<MODE_16, 16>(L, ws, st, num_sms, ev);

@@ -131,6 +131,11 @@ extern long long g_launches;
 
 int tm_encode_2d(CUtensorMap* tm, int dtype, const void* base, uint64_t d0, uint64_t d1, uint64_t stride1_bytes,
                  uint32_t b0, uint32_t b1);   // 2-D tiled tensor map, SWIZZLE_128B (api.cu)
+// per-device launch set-up (api.cu), safe to call from several host threads.  kernel_smem raises fn's dynamic
+// shared-memory limit on the current device when `bytes` exceeds what was set there before (`what` labels a failure);
+// device_sms returns the SM count of `dev`.  Both return a negative B200_ERR_* code on failure.
+int kernel_smem(const void* fn, int bytes, const char* what);
+int device_sms(int dev);
 Workspace* get_workspace(int device);
 int ensure_workspace(Workspace* ws, const b200moe_layer* L, int64_t tokens, int top_k, bool may_alloc);
 void release_workspace(Workspace* ws);

@@ -445,19 +445,14 @@ int launch_prep(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const vo
                 int M, int k, int tn_max) {
   const int n_slots = M * k;
   // dynamic shared memory: warp-private rank counters [warps][E] (E <= 1024: 64 KB)
-  static bool sort_attr = false;
-  if (!sort_attr) {
-    cudaFuncSetAttribute(route_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (SORT_THREADS / 32) * MAX_EXPERTS * 4);
-    sort_attr = true;
-  }
+  const int wc_max = (SORT_THREADS / 32) * MAX_EXPERTS * 4;
+  int rc = kernel_smem(reinterpret_cast<const void*>(route_sort_kernel), wc_max, "cudaFuncSetAttribute(route_sort)");
+  if (rc) return rc;
   const size_t wc_bytes = (size_t)(SORT_THREADS / 32) * L->E * 4;
   if (n_slots >= 8192 && ws->sort_hist) {
     // prefill-class batch: histogram / scan / scatter over up to 128 CTAs (same (expert, slot) order)
-    static bool scat_attr = false;
-    if (!scat_attr) {
-      cudaFuncSetAttribute(route_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (SORT_THREADS / 32) * MAX_EXPERTS * 4);
-      scat_attr = true;
-    }
+    rc = kernel_smem(reinterpret_cast<const void*>(route_scatter_kernel), wc_max, "cudaFuncSetAttribute(route_scatter)");
+    if (rc) return rc;
     int n_ctas = (n_slots + 1023) / 1024;
     if (n_ctas > SORT_MAX_CTAS) n_ctas = SORT_MAX_CTAS;
     const int spc = (((n_slots + n_ctas - 1) / n_ctas) + 31) & ~31;

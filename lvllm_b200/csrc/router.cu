@@ -374,12 +374,8 @@ int b200_router_topk(void* stream, const void* hidden, int act_dtype, const void
   a.shared_w = shared_weight;
   const size_t route_scratch = (size_t)(R_THREADS / 32) * 2 * a.Epad * 4;
   const size_t smem = 1024 + (size_t)R_STAGES * (R_A_BYTES + TN * 128) + (size_t)TN * a.Epad * 4 + route_scratch;
-  static size_t smem_set = 0;
-  if (smem > smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(router_gemm_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(router)");
-    smem_set = smem;
-  }
+  if ((rc = kernel_smem(reinterpret_cast<const void*>(router_gemm_topk_kernel), (int)smem, "cudaFuncSetAttribute(router)")))
+    return rc;
   router_gemm_topk_kernel<<<dim3(KS, TT, EZ), R_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
