@@ -89,8 +89,11 @@ struct FCfg {
   static constexpr int MMA_THREADS = WD ? 256 : 128;
   static constexpr int NTHREADS = MMA_WARP0 * 32 + MMA_THREADS;
   // WD: registers after setmaxnreg (consumers / everything else); the pool is the launch's 65536 / NTHREADS rounded
-  // down to 8 per thread
-  static constexpr int REG_MMA = 120, REG_REST = 80;
+  // down to 8 per thread.  At 64 columns a consumer holds 64 fp32 accumulators, two slices of A fragments (16) and the
+  // next slice's nibble words (8): below 144 ptxas serialises the wgmmas (C7512).  The narrower instantiations pipeline at
+  // 120 and keep 80 for the other warps.
+  static constexpr int REG_MMA = (WD && TNMAX == 64) ? 144 : 120;
+  static constexpr int REG_REST = (WD && TNMAX == 64) ? 64 : 80;
   static_assert(!WD || REG_MMA * MMA_THREADS + REG_REST * (NTHREADS - MMA_THREADS) <= (65536 / NTHREADS) / 8 * 8 * NTHREADS,
                 "register split exceeds the launch allocation");
   static constexpr int BUFCOLS = 2 * TNMAX;       // gate + up accumulators (GEMM2 uses the first TNMAX)
@@ -127,8 +130,20 @@ struct __align__(16) FTables {
 };
 static_assert(sizeof(FTables) <= 24 * 1024, "FTables too large");
 
+// The 4-bit consumer warpgroups time out through a call (OUTLINED_TRAP): ptxas gives a setmaxnreg.inc region its raised
+// register count only when no trap instruction lies inside it; otherwise it allocates the region at about the launch's
+// count, and the 64-column consumers serialise their wgmmas for want of registers.
+__device__ __noinline__ void f_timeout() { __trap(); }
+template <bool OUTLINED_TRAP = false>
 B200_DEVICE void f_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
+  if (OUTLINED_TRAP) {   // the call stays out of the polling loop
+    bool done;
+    while (!(done = mbar_try_wait(bar, parity)) && ++spins <= (1u << 27)) {
+    }
+    if (!done) f_timeout();
+    return;
+  }
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > (1u << 27)) __trap();
   }
@@ -246,28 +261,69 @@ B200_DEVICE uint32_t lds_u8(uint32_t addr) {
   asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
   return v;
 }
-// scale of row r for the 16 columns [32 grp + 16 sub, +16) (sc: shared-memory address of the tile's scales)
+// raw scale of row r for the 16 columns [32 grp + 16 sub, +16) (sc: shared-memory address of the tile's scales) and its
+// conversion to an fp16 pair
 template <int WQ>
-B200_DEVICE __half2 w4_scale(uint32_t sc, int grp, int sub, int r) {
+B200_DEVICE uint32_t w4_scale_ld(uint32_t sc, int grp, int sub, int r) {
+  if (WQ == 1) return lds_u16(sc + (grp * 128 + r) * 2);
+  if (WQ == 2) return lds_u8(sc + (2 * grp + sub) * 128 + r);
+  return lds_u8(sc + grp * 128 + r);
+}
+template <int WQ>
+B200_DEVICE __half2 w4_scale(uint32_t raw) {
   if (WQ == 1) {
-    const uint16_t b = (uint16_t)lds_u16(sc + (grp * 128 + r) * 2);
+    const uint16_t b = (uint16_t)raw;
     return __half2half2(*reinterpret_cast<const __half*>(&b));
   }
   if (WQ == 2) {
-    const __half_raw h = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)lds_u8(sc + (2 * grp + sub) * 128 + r), __NV_E4M3);
+    const __half_raw h = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)raw, __NV_E4M3);
     return __half2half2(*reinterpret_cast<const __half*>(&h));
   }
   // e8m0 -> fp16 2^(E-127): exponent field E-112 clamped to [0,30] (scales < 2^-14 flush to 0)
-  int f = (int)lds_u8(sc + grp * 128 + r) - 112;
+  int f = (int)raw - 112;
   f = f < 0 ? 0 : (f > 30 ? 30 : f);
   const uint16_t bits = (uint16_t)(f << 10);
   return __half2half2(*reinterpret_cast<const __half*>(&bits));
 }
 
-// k-iterations [ki0, ki1) of one tile at NN token columns: per k16 slice, convert the gate and up fragments of this
-// warpgroup's rows, then issue their two MMAs (A registers, B = token tile of the stage).  The conversion of a slice runs
-// while the MMAs of the previous one are in flight (wait_group 1); a stage is released once the MMAs of the next one
-// have been waited for, the last one of the tile after wait_group 0.
+// The shared-memory words one thread needs for a k16 slice: rows r0 and r0 + 8 of the gate (na = 0) and up (na = 1) tile.
+// They are loaded one slice ahead, so that their load latency is hidden behind the conversion of the previous slice.  SC:
+// the scales are loaded ahead too.  At 64 columns the accumulators leave no registers for them, and they are loaded with
+// the conversion instead, whose nibble arithmetic covers part of their latency.
+struct W4Slice {
+  uint2 q0[2], q1[2];
+  uint32_t s0[2], s1[2];
+};
+template <int WQ, bool SC>
+B200_DEVICE void w4_load(W4Slice& v, uint32_t raw, int tile_bytes, int kk, int ks, int r0) {
+  const int grp = ks >> 1, sub = ks & 1;
+#pragma unroll
+  for (int na = 0; na < 2; ++na) {
+    const uint32_t tile = raw + (kk * 2 + na) * tile_bytes;
+    v.q0[na] = lds_u2(tile + (grp * 128 + r0) * 16 + sub * 8);
+    v.q1[na] = lds_u2(tile + (grp * 128 + r0 + 8) * 16 + sub * 8);
+    if (SC) {
+      v.s0[na] = w4_scale_ld<WQ>(tile + 4096, grp, sub, r0);
+      v.s1[na] = w4_scale_ld<WQ>(tile + 4096, grp, sub, r0 + 8);
+    }
+  }
+}
+template <int WQ, bool SC>
+B200_DEVICE void w4_convert(uint32_t (&f)[2][4], const W4Slice& v, uint32_t raw, int tile_bytes, int kk, int ks, int r0,
+                            int t) {
+  const int grp = ks >> 1, sub = ks & 1;
+#pragma unroll
+  for (int na = 0; na < 2; ++na) {
+    const uint32_t sc = raw + (kk * 2 + na) * tile_bytes + 4096;
+    const __half2 s0 = w4_scale<WQ>(SC ? v.s0[na] : w4_scale_ld<WQ>(sc, grp, sub, r0));
+    const __half2 s1 = w4_scale<WQ>(SC ? v.s1[na] : w4_scale_ld<WQ>(sc, grp, sub, r0 + 8));
+    f[na][0] = w4_pair<WQ>(v.q0[na].x, t, s0);
+    f[na][1] = w4_pair<WQ>(v.q1[na].x, t, s1);
+    f[na][2] = w4_pair<WQ>(v.q0[na].y, t, s0);
+    f[na][3] = w4_pair<WQ>(v.q1[na].y, t, s1);
+  }
+}
+
 // pins the accumulators in their registers across the asynchronous MMAs: without it the compiler may rematerialise or move
 // them, and ptxas then serialises every wgmma
 template <int N>
@@ -277,53 +333,65 @@ B200_DEVICE void acc_fence(float (&acc)[2][N]) {
 #pragma unroll
     for (int i = 0; i < N; ++i) asm volatile("" : "+f"(acc[na][i])::"memory");
 }
+// a use of one slice's A fragments at the point from which they may be overwritten
+B200_DEVICE void frag_hold(uint32_t (&f)[2][4]) {
+#pragma unroll
+  for (int na = 0; na < 2; ++na)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(f[na][i]));
+}
 
+// k-iterations [ki0, ki1) of one tile at NN token columns: per k16 slice, convert the gate and up fragments of this
+// warpgroup's rows, then issue their two MMAs (A registers, B = token tile of the stage).  Two slices are in flight: the
+// conversion of slice n runs while the MMAs of slice n - 1 execute (wait_group 1), with the shared-memory words of slice
+// n + 1 already requested.  A stage is released once the MMAs of the next one have been waited for, the last one of the
+// tile after wait_group 0.
 template <class C, int NN>
 B200_DEVICE void w4_tile(const FusedArgs& a, FTables* tb, const uint8_t* smem, int KB, int ki0, int ki1,
                          float (&acc)[2][C::TN / 2], uint32_t& itc) {
   constexpr int WQ = C::WD;
+  constexpr bool SC = C::TN < 64;
   const int lane = threadIdx.x & 31;
   const int r0 = (((int)threadIdx.x >> 7) - C::MMA_WARP0 / 4) * 64 + (((int)threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
   const int t = lane & 3;
   const bool lead = (threadIdx.x & 127) == 0;
   const uint32_t smem_u = smem_u32(smem);
   int pend = -1;   // stage whose last MMAs may still be in flight
+  // A fragments, double-buffered by slice parity: slice n converts into fa[n & 1] while the MMAs of slice n - 1 still
+  // read fa[(n - 1) & 1].  frag_hold below keeps the older buffer live until those MMAs have been waited for, so the
+  // register allocator has to give the two buffers distinct registers and ptxas need not serialise the wgmmas.
+  uint32_t fa[2][2][4] = {};
   acc_fence(acc);
   for (int ki = ki0; ki < ki1; ++ki, ++itc) {
     const int s = itc % C::STAGES;
-    f_wait(&tb->full[s], (itc / C::STAGES) & 1);
+    f_wait<true>(&tb->full[s], (itc / C::STAGES) & 1);
     const int kb0 = ki * 2;
     const int nkb = (KB - kb0) < 2 ? (KB - kb0) : 2;
     const uint32_t raw = smem_u + s * C::STAGE;
     const uint32_t sb = raw + C::A_STAGE;
     for (int kk = 0; kk < nkb; ++kk) {
       const uint32_t bbase = sb + kk * (uint32_t)((NN >> 3) * 1024);
+      W4Slice cur;
+      w4_load<WQ, SC>(cur, raw, a.w4_tile_bytes, kk, 0, r0);
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
-        const int grp = ks >> 1, sub = ks & 1;
-        uint32_t fa[2][4];
-#pragma unroll
-        for (int na = 0; na < 2; ++na) {
-          const uint32_t tile = raw + (kk * 2 + na) * a.w4_tile_bytes;
-          const uint2 q0 = lds_u2(tile + (grp * 128 + r0) * 16 + sub * 8);
-          const uint2 q1 = lds_u2(tile + (grp * 128 + r0 + 8) * 16 + sub * 8);
-          const __half2 s0 = w4_scale<WQ>(tile + 4096, grp, sub, r0), s1 = w4_scale<WQ>(tile + 4096, grp, sub, r0 + 8);
-          fa[na][0] = w4_pair<WQ>(q0.x, t, s0);
-          fa[na][1] = w4_pair<WQ>(q1.x, t, s1);
-          fa[na][2] = w4_pair<WQ>(q0.y, t, s0);
-          fa[na][3] = w4_pair<WQ>(q1.y, t, s1);
-        }
+        W4Slice nxt;
+        if (ks < 3) w4_load<WQ, SC>(nxt, raw, a.w4_tile_bytes, kk, ks + 1, r0);
+        uint32_t (&f)[2][4] = fa[ks & 1];
+        w4_convert<WQ, SC>(f, cur, raw, a.w4_tile_bytes, kk, ks, r0, t);
         const uint64_t bd = wgmma_desc_sw128(bbase + ks * 32, 1024);
         const uint32_t accum = (ki > ki0 || kk > 0 || ks > 0) ? 1u : 0u;
         wgmma_fence();
-        WgmmaRS<NN, 0>::mma(acc[0], fa[0], bd, accum);
-        WgmmaRS<NN, 0>::mma(acc[1], fa[1], bd, accum);
+        WgmmaRS<NN, 0>::mma(acc[0], f[0], bd, accum);
+        WgmmaRS<NN, 0>::mma(acc[1], f[1], bd, accum);
         wgmma_commit();
         wgmma_wait<1>();
+        frag_hold(fa[(ks + 1) & 1]);   // the previous slice's MMAs are complete: its buffer may be overwritten now
         if (pend >= 0) {
           if (lead) mbar_arrive(&tb->empty[pend]);
           pend = -1;
         }
+        if (ks < 3) cur = nxt;
       }
     }
     pend = s;
@@ -360,14 +428,14 @@ B200_DEVICE void w4_consumer(const FusedArgs& a, FTables* tb, const uint8_t* sme
       switch (tn) {
         case 16:
           w4_tile<C, 16>(a, tb, smem, KB, k0, k1, acc, itc);
-          f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+          f_wait<true>(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
           xch_store_frag<16>(base, half, acc[0]);
           xch_store_frag<16>(base + TNMAX, half, acc[1]);
           break;
         case 32:
           if constexpr (TNMAX >= 32) {
             w4_tile<C, 32>(a, tb, smem, KB, k0, k1, acc, itc);
-            f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+            f_wait<true>(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
             xch_store_frag<32>(base, half, acc[0]);
             xch_store_frag<32>(base + TNMAX, half, acc[1]);
           }
@@ -375,7 +443,7 @@ B200_DEVICE void w4_consumer(const FusedArgs& a, FTables* tb, const uint8_t* sme
         case 48:
           if constexpr (TNMAX >= 48) {
             w4_tile<C, 48>(a, tb, smem, KB, k0, k1, acc, itc);
-            f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+            f_wait<true>(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
             xch_store_frag<48>(base, half, acc[0]);
             xch_store_frag<48>(base + TNMAX, half, acc[1]);
           }
@@ -383,7 +451,7 @@ B200_DEVICE void w4_consumer(const FusedArgs& a, FTables* tb, const uint8_t* sme
         default:
           if constexpr (TNMAX >= 64) {
             w4_tile<C, 64>(a, tb, smem, KB, k0, k1, acc, itc);
-            f_wait(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
+            f_wait<true>(&tb->tempty[buf], ((acc_it / C::NBUF) & 1) ^ 1);
             xch_store_frag<64>(base, half, acc[0]);
             xch_store_frag<64>(base + TNMAX, half, acc[1]);
           }
@@ -1120,9 +1188,10 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
           if (finalize) __threadfence();  // acquire side of the contributor counter
         }
         // Finalisation runs in blocks of FB token columns so that every array stays in registers: the fix-up warps of
-        // the 4-bit variants have 80 registers per thread, and whole-tile arrays (acc[2][32] + tmp[4][32]) would live in
-        // local memory, serialising the L2 round trips.
-        constexpr int FB = WD ? 8 : 16;
+        // the 4-bit variants have 80 registers per thread (64 at 64 columns), and whole-tile arrays (acc[2][32] +
+        // tmp[4][32]) would live in local memory, serialising the L2 round trips.  The blocking does not change the order
+        // in which a column's partials are summed.
+        constexpr int FB = WD ? (TNMAX == 64 ? 4 : 8) : 16;
         if (finalize) {
           const float* own = a.partials + ((size_t)(4 * G * 2) + (size_t)cta * F_QD + qe) * (size_t)(2 * TNMAX * 128);
           // NVFP4 per-expert global scales (gate / up of w13, w2): linear, applied once to the reduced sums

@@ -145,9 +145,15 @@ def main():
     g = torch.Generator().manual_seed(0)
     mix = dict(fmt="int4", E=8, k=2, H=4096, I=14336)
     uni = torch.stack([torch.arange(64) * 2 % 8, (torch.arange(64) * 2 + 1) % 8], 1).int()   # 16 rows per expert
+    # the benchmark's routing in closed form: every token picks expert 0, and expert 1 or (one token in 8) expert 2 ->
+    # chunks of 64, 56 and 8 rows, run by the 64-column instantiation
+    conc = torch.stack([torch.zeros(64, dtype=torch.long), torch.where(torch.arange(64) % 8 == 0, 2, 1)], 1).int()
     cases = [
         ("mixtral_int4_m64_bench_routing", mix, lambda: bench_like_ids(dev)),
         ("mixtral_int4_m64_uniform", mix, lambda: uni),
+        ("mixtral_int4_m64_concentrated", mix, lambda: conc),
+        ("mixtral_mxfp4_m64_concentrated", dict(mix, fmt="mxfp4"), lambda: conc),
+        ("mixtral_nvfp4_m64_concentrated", dict(mix, fmt="nvfp4"), lambda: conc),
         ("mixtral_int4_m1", mix, lambda: random_ids(1, 8, 2, g)),
         ("mixtral_int4_m16", mix, lambda: random_ids(16, 8, 2, g)),
         ("mixtral_int4_m256", mix, lambda: random_ids(256, 8, 2, g)),

@@ -1,6 +1,7 @@
 """Count the SASS mnemonics that prove the Hopper data path per kernel of lvllm_b200/libb200moe.so (cuobjdump -sass):
 warpgroup MMAs (HGMMA 16-bit / QGMMA fp8), tensor-map TMA (UTMALDG), bulk async copies (UBLKCP), cp.async (LDGSTS), and the
-warp-level HMMA / IMMA / QMMA that must NOT appear.  usage: python tools/sass_evidence.py"""
+warp-level HMMA / IMMA / QMMA that must NOT appear.  WGDEPBAR1 counts `WARPGROUP.DEPBAR.LE gsb0, 0x1`: a wait that leaves one
+wgmma group in flight, i.e. MMAs that ptxas did not serialise.  usage: python tools/sass_evidence.py"""
 import collections
 import os
 import re
@@ -10,6 +11,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "lvllm_b200", "libb200moe.so")
 PAT = re.compile(r"\b(HGMMA|QGMMA|UTMALDG|UTMASTG|UBLKCP|LDGSTS|HMMA|IMMA|QMMA|F2FP)\b")
+DEPBAR1 = re.compile(r"WARPGROUP\.DEPBAR\.LE gsb0, 0x1\b")
 
 
 def main():
@@ -27,6 +29,8 @@ def main():
         m = PAT.search(ln)
         if m:
             per[cur][m.group(1)] += 1
+        if DEPBAR1.search(ln):
+            per[cur]["WGDEPBAR1"] += 1
     try:
         names = subprocess.run(["c++filt"], input="\n".join(per), stdout=subprocess.PIPE, text=True).stdout.splitlines()
     except OSError:
