@@ -210,11 +210,30 @@ int b200_mla_decode_spec(void* stream, const void* q_nope, const void* q_pe, int
                          const int32_t* page_table, int batch, int q_len, int num_heads, int page_size, int max_pages,
                          float sm_scale, int num_splits, void* workspace, void* out, float* lse, const void* w_uv,
                          void* out_v);
+/* Sparse MLA decode (DeepSeek-V3.2 / GLM-5 layers, config.index_topk): query token t attends only to the keys its lightning
+ * indexer selected.  Replaces the reference's triton_convert_req_index_to_global_index (v1/attention/backends/mla/
+ * sparse_utils.py:120) followed by the FlashMLA sparse decode (flashmla_sparse.py:587-611, 763-830): the conversion is fused
+ * into the kernel's gather.  q_nope [T,Hq,512], q_pe [T,Hq,64] bf16 (T = num_tokens query tokens; the draft tokens of a
+ * request are simply tokens with the same req_id); topk_indices int32 [T, topk], request-local key positions, entry j of
+ * token t is key row page_table[req_id[t]][idx / page_size] * page_size + idx % page_size; an entry with idx < 0 or
+ * idx / page_size >= max_pages is skipped.  req_id int32 [T] (rows of page_table, int32 [*, max_pages]).  kv_dtype 0: bf16
+ * cache [pages, page_size, 576]; kv_dtype 2: fp8_ds_mla cache [pages, page_size, 656] bytes (512 e4m3 | 4 fp32 scales, one per
+ * 128 dims | 64 bf16 rope dims, flashmla_sparse.py:63-72), widened to bf16(float(e4m3) * scale) on the way into shared
+ * memory.  out bf16 [T,Hq,512], lse f32 [T,Hq] (natural log) or NULL; a token with no valid entry gets out = 0, lse = -inf.
+ * w_uv / out_v as in b200_mla_decode_spec.  Workspace: b200_mla_decode_workspace_bytes(num_tokens, num_heads, num_splits).
+ * B200_ERR_INVALID, nothing launched: kv_dtype other than 0 / 2, num_heads > 128, topk < 1, a NULL required pointer,
+ * num_splits <= 0, or num_splits > 512 with w_uv. */
+int b200_mla_decode_sparse(void* stream, const void* q_nope, const void* q_pe, const void* kv_cache, int kv_dtype,
+                           const int32_t* topk_indices, int topk, const int32_t* req_id, const int32_t* page_table,
+                           int max_pages, int num_tokens, int num_heads, int page_size, float sm_scale, int num_splits,
+                           void* workspace, void* out, float* lse, const void* w_uv, void* out_v);
 /* The MLA decode kernel's neighbours (SURVEY.md 8f row 3), bf16:
  *  b200_mla_rope_cache_write  RoPE of q_pe [T,Hq,64] and k_pe [T,64] in place (rotary_embedding/base.py:161-201; cos_sin_cache
  *      bf16 [max_pos,64] = cos | sin; is_neox 0 = GPT-J pairs (DeepSeek), 1 = NeoX halves) fused with concat_and_cache_mla
  *      (csrc/libtorch_stable/cache_kernels.cu:403-444): row slot_mapping[t] (i64, < 0 = padded token) of the paged latent
  *      cache [blocks*block_size, 576] <- [kv_c[t] (512) | rotated k_pe[t]]; kv_dtype 1 = e4m3 cache storing value / kv_scale;
+ *      kv_dtype 2 = fp8_ds_mla cache [blocks*block_size, 656] bytes (concat_and_cache_ds_mla_kernel, cache_kernels.cu:496-590:
+ *      per 128-dim tile scale = max(amax / 448, FLT_MIN) as fp32 and e4m3(value / scale); kv_scale unused);
  *  b200_mla_q_absorb          ql_nope [T,Hq,512] = q_nope [T,Hq,128] x W_UK_T [Hq,128,512]  (mla_attention.py:875-893);
  *  b200_mla_decode_vup        b200_mla_decode_ex whose split merge is fused with the v up-projection
  *      out_v [B,Hq,128] = o [B,Hq,512] x W_UV [Hq,512,128] (mla_attention.py:1154-1176); out_latent (optional) = o. */

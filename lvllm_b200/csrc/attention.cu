@@ -217,6 +217,23 @@ __global__ void __launch_bounds__(128) mla_merge_kernel(const float* __restrict_
   if (lse && tid == 0) lse[w] = (lsum > 0.f) ? (mx * 0.6931471805599453f + logf(lsum)) : -CUDART_INF_F;
 }
 
+// merge of the MLA decode kernel's partials over query rows x heads: fused with the v up-projection when w_uv is given
+// (mla_aux.cu), mla_merge_kernel up to 512 splits, decode_merge_kernel above
+static int mla_merge(cudaStream_t st, const float* po, const float* pml, int rows, int num_heads, int num_splits, void* out,
+                     float* lse, const void* w_uv, void* out_v) {
+  if (w_uv)
+    launch_mla_merge_vup(st, po, pml, rows, num_splits, num_heads, w_uv, out_v, out, lse);
+  else if (num_splits <= 512)
+    mla_merge_kernel<<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
+  else
+    decode_merge_kernel<512><<<(rows * num_heads + 3) / 4, 128, 0, st>>>(po, pml, rows * num_heads, num_splits,
+                                                                        reinterpret_cast<__nv_bfloat16*>(out), lse);
+  ++g_launches;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "mla merge launch");
+  return 0;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -269,17 +286,27 @@ int b200_mla_decode_spec(void* stream, const void* q_nope, const void* q_pe, int
   int rc = launch_mla_tc(st, q_nope, q_pe, kv_cache, seq_lens, page_table, batch, q_len, num_heads, page_size, max_pages,
                          sm_scale, num_splits, po, pml, kv_dtype, q_dtype, descale_q, descale_k);
   if (rc) return rc;
-  if (w_uv)   // split merge fused with the v up-projection (mla_aux.cu)
-    launch_mla_merge_vup(st, po, pml, rows, num_splits, num_heads, w_uv, out_v, out, lse);
-  else if (num_splits <= 512)
-    mla_merge_kernel<<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
-  else
-    decode_merge_kernel<512><<<(rows * num_heads + 3) / 4, 128, 0, st>>>(po, pml, rows * num_heads, num_splits,
-                                                                        reinterpret_cast<__nv_bfloat16*>(out), lse);
-  ++g_launches;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "mla merge launch");
-  return 0;
+  return mla_merge(st, po, pml, rows, num_heads, num_splits, out, lse, w_uv, out_v);
+}
+
+int b200_mla_decode_sparse(void* stream, const void* q_nope, const void* q_pe, const void* kv_cache, int kv_dtype,
+                           const int32_t* topk_indices, int topk, const int32_t* req_id, const int32_t* page_table,
+                           int max_pages, int num_tokens, int num_heads, int page_size, float sm_scale, int num_splits,
+                           void* workspace, void* out, float* lse, const void* w_uv, void* out_v) {
+  if (!q_nope || !q_pe || !kv_cache || !topk_indices || !req_id || !page_table || !workspace || num_tokens <= 0 ||
+      num_heads <= 0 || num_heads > 128 || topk < 1 || page_size <= 0 || max_pages <= 0 || num_splits <= 0 ||
+      (kv_dtype != 0 && kv_dtype != 2) || (w_uv ? (!out_v || num_splits > 512) : !out)) {
+    set_error("b200_mla_decode_sparse: bad argument (kv_dtype 0 or 2, num_heads <= 128, topk >= 1; out, or with w_uv out_v "
+              "and num_splits <= 512)");
+    return B200_ERR_INVALID;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* po = reinterpret_cast<float*>(workspace);
+  float* pml = po + (size_t)num_tokens * num_heads * num_splits * 512;
+  const int rc = launch_mla_sparse_tc(st, q_nope, q_pe, kv_cache, kv_dtype == 2, topk_indices, topk, req_id, page_table,
+                                      max_pages, num_tokens, num_heads, page_size, sm_scale, num_splits, po, pml);
+  if (rc) return rc;
+  return mla_merge(st, po, pml, num_tokens, num_heads, num_splits, out, lse, w_uv, out_v);
 }
 
 int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void* v_cache, const int32_t* seq_lens,

@@ -22,6 +22,16 @@
 // varies with the value-dim part in blockIdx.y, so the CTAs reading the same KV tile are scheduled together.  Each
 // accumulator row masks with its own key count; Q = 1 is the single-token decode (one q-group, rows = heads).
 //
+// Sparse decode (DeepSeek-V3.2 / GLM-5 layers with a lightning indexer): query token t attends only to the keys its
+// indexer picked, topk_indices[t, 0 .. topk), request-local positions of request req_id[t] (-1 = no key).  A CTA is (token,
+// split over index tiles, value-dim quarter); a tile is 128 consecutive entries of the token's index row, and the loaders
+// take each key row from the index (page_table[req_id[t]][idx / page] * page + idx % page, the reference's
+// triton_convert_req_index_to_global_index, v1/attention/backends/mla/sparse_utils.py:120, fused into the gather).  An entry
+// with idx < 0 or idx / page >= max_pages is invalid: its row is zero-filled and its column masked for every row of the CTA
+// through a per-tile 128-bit mask the loaders publish in shared memory.  The cache is bf16 (576 elements per token) or
+// fp8_ds_mla (656 bytes per token: 512 e4m3, four fp32 scales, one per 128 dims, 64 bf16 rope dims; reference
+// v1/attention/backends/mla/flashmla_sparse.py:63-72), widened to bf16 by the loaders.
+//
 // Warp roles (384 threads): warps 0-3 / 4-7 consumer warpgroups (MMA + softmax + epilogue), warps 8-11 loaders
 // (16-byte gathers of q rows / paged KV rows -> swizzled smem, generic->async proxy fence).
 // The op contract is reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262.
@@ -48,6 +58,10 @@ struct MlaBars {
   uint64_t full[MLA_KB], empty[MLA_QSTAGES];
   uint64_t s_full, o_full;   // QK^T / PV of the tile complete in both warpgroups: its blocks may be refilled
   int8_t row_off[128];       // SPEC: MMA row r sees row_off[r] keys fewer than the q-group's last draft token
+  // SPARSE: the valid columns of tile ti in kvalid[ti & 1]; loader warp w publishes word w, bit 4u + r = column
+  // 16u + 4w + r, and arrives on v_full once the word is written
+  uint64_t v_full;
+  uint32_t kvalid[2][4];
 };
 
 B200_DEVICE void mla_wait(uint64_t* bar, uint32_t parity) {
@@ -74,19 +88,39 @@ B200_DEVICE uint4 fp8x8_to_bf16x8(uint2 v) {
   return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
+// eight e4m3 bytes of an fp8_ds_mla row -> eight bf16 bf16(float(e4m3) * scale): the fp32 product, rounded once to bf16
+B200_DEVICE uint4 fp8x8_scaled_to_bf16x8(uint2 v, float scale) {
+  const uint32_t w[2] = {v.x, v.y};
+  uint32_t o[4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)((w[i] >> (16 * h)) & 0xFFFFu), __NV_E4M3);
+      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+      const __nv_bfloat162 b = __floats2bfloat162_rn(__fmul_rn(f.x, scale), __fmul_rn(f.y, scale));
+      o[i * 2 + h] = *reinterpret_cast<const uint32_t*>(&b);
+    }
+  }
+  return make_uint4(o[0], o[1], o[2], o[3]);
+}
+
 // KV8: the latent cache is e4m3 (kv_cache_dtype "fp8": 576 bytes per token, half the HBM traffic of the bf16 cache;
 // reference fp8 dtypes backends/mla/cutlass_mla.py:44-45).  The loaders widen it to bf16 on the way into shared memory
 // (exact), so the tensor-core pipeline and its numerics are those of the bf16 kernel — P is NOT re-quantised to fp8.
 // q8: the queries are e4m3 too (the reference's fp8 test feeds fp8 q, tests/kernels/attention/test_cutlass_mla_decode.py:101-110).
 // SPEC: Q > 1 query tokens per request.  Without it every q-group expression below is a compile-time constant (Q = Qg = 1,
 // rows = heads, one limit for every row), which keeps the single-token decode free of the per-row bookkeeping.
-template <bool KV8, bool SPEC>
+// SPARSE: blockIdx.z is a query token, its keys come from topk_idx (see the header); with KV8 the cache is fp8_ds_mla (the
+// queries are bf16 then, q8 = 0).  The three trailing arguments are read by the sparse instantiations only.
+template <bool KV8, bool SPEC, bool SPARSE>
 __global__ void __launch_bounds__(MLA_THREADS, 1)
     mla_decode_tc_kernel(const void* __restrict__ q_nope_v, const void* __restrict__ q_pe_v,
                          const void* __restrict__ kv_v, const int32_t* __restrict__ seq_lens,
                          const int32_t* __restrict__ page_table, int Hq, int page_size, int max_pages,
                          float scale_log2, int num_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
-                         int q8, float out_scale, int tiles_per_cta, int Q_, int Qg_) {
+                         int q8, float out_scale, int tiles_per_cta, int Q_, int Qg_,
+                         const int32_t* __restrict__ topk_idx, const int32_t* __restrict__ req_id, int topk) {
   const __nv_bfloat16* q_nope = reinterpret_cast<const __nv_bfloat16*>(q_nope_v);
   const __nv_bfloat16* q_pe = reinterpret_cast<const __nv_bfloat16*>(q_pe_v);
   const __nv_bfloat16* kv = reinterpret_cast<const __nv_bfloat16*>(kv_v);
@@ -104,7 +138,8 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
   const int nrows = qn * Hq;                         // MMA rows that carry a query
   const size_t row0 = (size_t)(b * Q + qg * Qg) * Hq;   // q / output row of MMA row 0
   // keys of the group's last draft token: the most any row of this CTA sees (all of them when Q = 1)
-  const int S = SPEC ? seq_lens[b] - Q + qg * Qg + qn : seq_lens[b];
+  // (SPARSE: the entries of the token's index row)
+  const int S = SPARSE ? topk : SPEC ? seq_lens[b] - Q + qg * Qg + qn : seq_lens[b];
   const int t_first = split * tiles_per_cta * MLA_TOK;
   // this CTA walks n_tiles consecutive 128-token tiles of the request with an online softmax: O stays in registers,
   // partial (O, m, l) leave the CTA once
@@ -125,6 +160,7 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
     for (int i = 0; i < MLA_QSTAGES; ++i) mbar_init(&bars->empty[i], 2);   // one arrival per consumer warpgroup
     mbar_init(&bars->s_full, 2);
     mbar_init(&bars->o_full, 2);
+    if (SPARSE) mbar_init(&bars->v_full, 4);   // one arrival per loader warp
     fence_barrier_init();
   }
   // row r is draft token j = r / Hq of the group (rows past its last token take that token's limit)
@@ -150,6 +186,30 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
       // base pointers of this thread's 8 KV rows (paged)
       const __nv_bfloat16* krow[8];
       const uint8_t* krow8[8];
+      float kscale[8][4];   // SPARSE && KV8: the row's four fp8_ds_mla scales
+      uint32_t vword = 0;   // SPARSE: this warp's word of the tile's valid mask
+      if (SPARSE) {
+        const int32_t* pt_row = page_table + (size_t)req_id[b] * max_pages;
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const int tt = r0 + 16 * u;
+          const int idx = tt < nt ? topk_idx[(size_t)b * topk + t0 + tt] : -1;
+          const bool ok = idx >= 0 && idx / page_size < max_pages;
+          const size_t row = ok ? (size_t)pt_row[idx / page_size] * page_size + idx % page_size : 0;
+          krow[u] = ok ? kv + row * 576 : nullptr;
+          krow8[u] = ok ? reinterpret_cast<const uint8_t*>(kv_v) + row * 656 : nullptr;
+          if (KV8) {
+            const float4 sc = ok ? __ldg(reinterpret_cast<const float4*>(krow8[u] + 512)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            kscale[u][0] = sc.x;
+            kscale[u][1] = sc.y;
+            kscale[u][2] = sc.z;
+            kscale[u][3] = sc.w;
+          }
+          // lanes 0, 8, 16, 24 hold rows 4 * (warp - 8) + 0..3 + 16u
+          const uint32_t bal = __ballot_sync(0xffffffffu, ok);
+          vword |= ((bal & 1u) | ((bal >> 7) & 2u) | ((bal >> 14) & 4u) | ((bal >> 21) & 8u)) << (4 * u);
+        }
+      } else {
 #pragma unroll
       for (int u = 0; u < 8; ++u) {
         const int tt = r0 + 16 * u;
@@ -163,6 +223,7 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
           krow8[u] = nullptr;
         }
       }
+      }
       if (KV8) {
         // e4m3 cache (and, with q8, e4m3 queries): 8-byte loads, widened to bf16 in registers, 16-byte stores into the
         // swizzled tiles; MLA_PF k-blocks of loads are kept in flight per thread (register ring)
@@ -173,9 +234,11 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
             const int r = r0 + 16 * u;
-            kreg[buf][u] = krow8[u] ? __ldg(reinterpret_cast<const uint2*>(krow8[u] + kb * 64 + c * 8)) : make_uint2(0u, 0u);
+            // fp8_ds_mla: the rope block (kb 8) is bf16 and goes in by cp.async
+            kreg[buf][u] = krow8[u] && !(SPARSE && kb == 8)
+                               ? __ldg(reinterpret_cast<const uint2*>(krow8[u] + kb * 64 + c * 8)) : make_uint2(0u, 0u);
             qreg[buf][u] = make_uint2(0u, 0u);
-            if (q8 && r < nrows)
+            if (!SPARSE && q8 && r < nrows)
               qreg[buf][u] = __ldg(reinterpret_cast<const uint2*>(kb < 8 ? qn8 + (row0 + r) * 512 + kb * 64 + c * 8
                                                                            : qp8 + (row0 + r) * 64 + c * 8));
           }
@@ -188,11 +251,15 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
           const int s = qit % MLA_QSTAGES, buf = j % MLA_PF;
           if (j + MLA_PF - 1 < MLA_KB) issue(j + MLA_PF - 1, (j + MLA_PF - 1) % MLA_PF);
           if (ti > 0) mla_wait(j < MLA_NO ? &bars->s_full : &bars->o_full, (ti - 1) & 1);   // the block's previous readers are done
+          if (SPARSE && j == 0 && lane == 0) {   // publish the mask once tile ti - 1's QK^T is done (see v_full)
+            bars->kvalid[ti & 1][warp - 8] = vword;
+            mbar_arrive(&bars->v_full);
+          }
           mla_wait(&bars->empty[s], ((qit / MLA_QSTAGES) & 1) ^ 1);
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
             const int r = r0 + 16 * u;
-            if (q8) {
+            if (!SPARSE && q8) {
               *reinterpret_cast<uint4*>(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(qreg[buf][u]);
             } else {
               const bool qok = r < nrows;
@@ -201,9 +268,16 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
                                                          : q_pe + (row0 + r) * 64 + c * 8);
               cp_async16(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16), qsrc, qok);
             }
-            *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(kreg[buf][u]);
+            if (!SPARSE)
+              *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(kreg[buf][u]);
+            else if (kb < 8)
+              *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) =
+                  fp8x8_scaled_to_bf16x8(kreg[buf][u], kscale[u][kb >> 1]);
+            else
+              cp_async16(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16),
+                         krow8[u] ? krow8[u] + 528 + c * 16 : kv_v, krow8[u] != nullptr);
           }
-          if (!q8) asm volatile("cp.async.wait_all;" ::: "memory");
+          if (SPARSE || !q8) asm volatile("cp.async.wait_all;" ::: "memory");
           fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
           mbar_arrive(&bars->full[kb]);
         }
@@ -213,6 +287,10 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
           const int kb = kb_of(j);
           const int s = qit % MLA_QSTAGES;
           if (ti > 0) mla_wait(j < MLA_NO ? &bars->s_full : &bars->o_full, (ti - 1) & 1);
+          if (SPARSE && j == 0 && lane == 0) {   // publish the mask once tile ti - 1's QK^T is done (see v_full)
+            bars->kvalid[ti & 1][warp - 8] = vword;
+            mbar_arrive(&bars->v_full);
+          }
           mla_wait(&bars->empty[s], ((qit / MLA_QSTAGES) & 1) ^ 1);
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
@@ -245,8 +323,15 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
     // row are a prefix of the sequence, so a row that sees nothing in the CTA's first tile sees nothing in any later one:
     // its m_run stays -inf (the lazy-rescale test compares NaN, which is false), it takes ms = 0 so that every P of it is
     // exp2(-inf) = 0 (exp2f never sees -inf - -inf), and it publishes exactly m = -inf, l = 0, O = 0, which the merges skip.
+    // SPARSE: the valid entries of a tile may be anywhere and a fully masked tile may come before a valid one; the masked
+    // logits are -inf and the same rules keep a row that has seen no valid key at m_run = -inf, P = 0, l = 0.
+    constexpr bool MASKED = SPEC || SPARSE;
     uint32_t qit = 0;
     for (int ti = 0; ti < n_tiles; ++ti) {
+      // SPARSE: wait for the tile's mask before the first wgmma of the tile.  The loaders publish the mask of tile ti + 1
+      // only after this warpgroup's QK^T of tile ti has completed, which needs every warp of it past this wait, so no
+      // warp can see the barrier two phases ahead.
+      if (SPARSE) mla_wait(&bars->v_full, ti & 1);
       const int nt = min(MLA_TOK, S - (t_first + ti * MLA_TOK));
       // valid tokens of the tile per row (row h0 + 8r), t < ntr[r]
       const int ntr[2] = {S - (t_first + ti * MLA_TOK) - bars->row_off[h0], S - (t_first + ti * MLA_TOK) - bars->row_off[h0 + 8]};
@@ -273,12 +358,21 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
         for (int i = 0; i < MLA_TOK / 2; ++i)
           if ((i >> 2) * 8 + quad * 2 + (i & 1) >= ntr[(i >> 1) & 1]) sacc[i] = -CUDART_INF_F;
       }
+      if (SPARSE) {   // column 8k + 2 quad + e is bit 4 (k / 2) + 2 (quad % 2) + e of mask word 2 (k % 2) + quad / 2
+        const uint32_t* vm = bars->kvalid[ti & 1];
+        const uint32_t v0 = vm[quad >> 1] >> (2 * (quad & 1)), v1 = vm[2 + (quad >> 1)] >> (2 * (quad & 1));
+#pragma unroll
+        for (int i = 0; i < MLA_TOK / 2; ++i) {
+          const int k = i >> 2;
+          if (!((((k & 1) ? v1 : v0) >> (4 * (k >> 1) + (i & 1))) & 1u)) sacc[i] = -CUDART_INF_F;
+        }
+      }
       // row maxima over the valid tokens of the tile: own columns, then the quad
       float m[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
       for (int i = 0; i < MLA_TOK / 2; ++i) {
         const int t = (i >> 2) * 8 + quad * 2 + (i & 1);
-        if (SPEC || t < nt) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], sacc[i]);
+        if (MASKED || t < nt) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], sacc[i]);
       }
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
@@ -302,15 +396,15 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
         }
         // SPEC: a row with no visible key so far (m_run = -inf) takes ms = 0, so that its masked logits give
         // exp2(-inf - 0) = 0 and never -inf - -inf
-        ms[r] = SPEC && m_run[r] == -CUDART_INF_F ? 0.f : m_run[r] * scale_log2;
+        ms[r] = MASKED && m_run[r] == -CUDART_INF_F ? 0.f : m_run[r] * scale_log2;
       }
       // P = exp2(s*scale - m*scale) -> bf16 pairs: the accumulator fragment of 16 tokens IS the A fragment of a k-step
       uint32_t pa[MLA_TOK / 16][4];
 #pragma unroll
       for (int i = 0; i < MLA_TOK / 2; i += 2) {
         const int t = (i >> 2) * 8 + quad * 2, r = (i >> 1) & 1;
-        const float p0 = (SPEC || t < nt) ? exp2f(fmaf(sacc[i], scale_log2, -ms[r])) : 0.f;
-        const float p1 = (SPEC || t + 1 < nt) ? exp2f(fmaf(sacc[i + 1], scale_log2, -ms[r])) : 0.f;
+        const float p0 = (MASKED || t < nt) ? exp2f(fmaf(sacc[i], scale_log2, -ms[r])) : 0.f;
+        const float p1 = (MASKED || t + 1 < nt) ? exp2f(fmaf(sacc[i + 1], scale_log2, -ms[r])) : 0.f;
         const __nv_bfloat162 pb = __floats2bfloat162_rn(p0, p1);
         // accumulate l from the ROUNDED probabilities so that O / l is consistent with the bf16 P used by the MMA
         l[r] += __low2float(pb) + __high2float(pb);
@@ -363,15 +457,36 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
   // descales (reference cutlass_mla.py: q_scale * k_scale folded into the softmax scale, k_scale into the output)
   const float sl2 = sm_scale * 1.4426950408889634f * (kv_fp8 ? descale_k * (q_fp8 ? descale_q : 1.f) : 1.f);
   const float osc = kv_fp8 ? descale_k : 1.f;
-  auto kern = q_len == 1 ? (!kv_fp8 ? mla_decode_tc_kernel<false, false> : mla_decode_tc_kernel<true, false>)
-                         : (!kv_fp8 ? mla_decode_tc_kernel<false, true> : mla_decode_tc_kernel<true, true>);
+  auto kern = q_len == 1 ? (!kv_fp8 ? mla_decode_tc_kernel<false, false, false> : mla_decode_tc_kernel<true, false, false>)
+                         : (!kv_fp8 ? mla_decode_tc_kernel<false, true, false> : mla_decode_tc_kernel<true, true, false>);
   const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc)");
   if (rc) return rc;
   kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size, max_pages, sl2, num_splits,
-                                            part_o, part_ml, kv_fp8 ? q_fp8 : 0, kv_fp8 ? osc : 1.f, tpc, q_len, Qg);
+                                            part_o, part_ml, kv_fp8 ? q_fp8 : 0, kv_fp8 ? osc : 1.f, tpc, q_len, Qg,
+                                            nullptr, nullptr, 0);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc launch");
+  return 0;
+}
+
+// sparse decode: one CTA row (grid.z) per query token; kv_ds_mla selects the fp8_ds_mla cache
+int launch_mla_sparse_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const void* kv, int kv_ds_mla,
+                         const int32_t* topk_idx, int topk, const int32_t* req_id, const int32_t* page_table, int max_pages,
+                         int num_tokens, int Hq, int page_size, float sm_scale, int num_splits, float* part_o,
+                         float* part_ml) {
+  dim3 grid(num_splits, MLA_PARTS, num_tokens);
+  const int tiles = (topk + MLA_TOK - 1) / MLA_TOK;
+  const int tpc = (tiles + num_splits - 1) / num_splits;
+  const float sl2 = sm_scale * 1.4426950408889634f;
+  auto kern = kv_ds_mla ? mla_decode_tc_kernel<true, false, true> : mla_decode_tc_kernel<false, false, true>;
+  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc sparse)");
+  if (rc) return rc;
+  kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, nullptr, page_table, Hq, page_size, max_pages, sl2, num_splits,
+                                            part_o, part_ml, 0, 1.f, tpc, 1, 1, topk_idx, req_id, topk);
+  ++g_launches;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc sparse launch");
   return 0;
 }
 

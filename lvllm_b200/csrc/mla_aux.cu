@@ -3,12 +3,16 @@
 //   mla_rope_cache_kernel   RoPE of q_pe / k_pe (reference rotary_embedding/base.py:161-201, common.py:146-185) fused with
 //                           concat_and_cache_mla (csrc/libtorch_stable/cache_kernels.cu:403-444): one launch per step
 //                           instead of rotary_embedding + concat_and_cache_mla, the rotated k_pe never returns to HBM twice;
+//                           With kv_dtype 2 the row is the 656-byte fp8_ds_mla entry of concat_and_cache_ds_mla_kernel
+//                           (cache_kernels.cu:496-590): 512 e4m3 | four fp32 scales, one per 128 dims | 64 bf16 rope dims;
 //   mla_absorb_kernel       ql_nope = q_nope x W_UK^T per head (mla_attention.py:875-893; torch.bmm in the reference);
 //   mla_merge_vup_kernel    the split merge of the decode kernel fused with the v up-projection (mla_attention.py:1154-1176):
 //                           the merged [512] latent output of a (request, head) never leaves shared memory.
 // All three are HBM / latency bound (W_UK_T and W_UV are 16.8 MB each for 128 heads): coalesced 16-byte loads, every
 // load of a thread's work issued before the first use, fp32 accumulation in a fixed order (deterministic).
 #include <math_constants.h>
+
+#include <cfloat>
 
 #include "common.cuh"
 #include "moe_internal.cuh"
@@ -22,7 +26,7 @@ __global__ void __launch_bounds__(128)
     mla_rope_cache_kernel(__nv_bfloat16* __restrict__ q_pe, __nv_bfloat16* __restrict__ k_pe,
                           const __nv_bfloat16* __restrict__ kv_c, const int64_t* __restrict__ positions,
                           const __nv_bfloat16* __restrict__ cos_sin, int is_neox, const int64_t* __restrict__ slot_mapping,
-                          void* __restrict__ kv_cache, int kv_fp8, float inv_scale, int Hq) {
+                          void* __restrict__ kv_cache, int kv_dtype, float inv_scale, int Hq) {
   const int t = blockIdx.x, tid = threadIdx.x;
   __shared__ float cs[64];   // cos[0..32) | sin[0..32) of this token's position
   if (tid < 64) cs[tid] = bf(cos_sin[(size_t)positions[t] * 64 + tid]);
@@ -30,7 +34,8 @@ __global__ void __launch_bounds__(128)
   // rotate the Hq query rope heads in place and the (single) key rope head; pair p of a head = (x1, x2):
   // GPT-J style (DeepSeek): elements (2p, 2p+1); NeoX style: (p, p + 32)
   const int64_t slot = slot_mapping ? slot_mapping[t] : -1;
-  uint8_t* crow8 = reinterpret_cast<uint8_t*>(kv_cache) + (size_t)(slot < 0 ? 0 : slot) * 576;
+  const bool kv_fp8 = kv_dtype == 1, ds_mla = kv_dtype == 2;
+  uint8_t* crow8 = reinterpret_cast<uint8_t*>(kv_cache) + (size_t)(slot < 0 ? 0 : slot) * (ds_mla ? 656 : 576);
   __nv_bfloat16* crow = reinterpret_cast<__nv_bfloat16*>(kv_cache) + (size_t)(slot < 0 ? 0 : slot) * 576;
   for (int i = tid; i < (Hq + 1) * 32; i += 128) {
     const int hd = i >> 5, p = i & 31;
@@ -43,7 +48,10 @@ __global__ void __launch_bounds__(128)
     x[i1] = o1;
     x[i2] = o2;
     if (is_k && slot >= 0) {
-      if (kv_fp8) {
+      if (ds_mla) {
+        reinterpret_cast<__nv_bfloat16*>(crow8 + 528)[i1] = o1;
+        reinterpret_cast<__nv_bfloat16*>(crow8 + 528)[i2] = o2;
+      } else if (kv_fp8) {
         crow8[512 + i1] = __nv_cvt_float_to_fp8(bf(o1) * inv_scale, __NV_SATFINITE, __NV_E4M3);
         crow8[512 + i2] = __nv_cvt_float_to_fp8(bf(o2) * inv_scale, __NV_SATFINITE, __NV_E4M3);
       } else {
@@ -52,7 +60,24 @@ __global__ void __launch_bounds__(128)
       }
     }
   }
-  if (slot >= 0) {
+  if (slot >= 0 && ds_mla) {
+    // threads 0-63 take 8 values each, a half-warp per 128-dim tile: scale = max(amax / 448, FLT_MIN), e4m3(value / scale)
+    if (tid < 64) {
+      const uint4 v = *reinterpret_cast<const uint4*>(kv_c + (size_t)t * 512 + tid * 8);
+      const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(&v);
+      float amax = 0.f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(bf(h[j])));
+#pragma unroll
+      for (int off = 8; off > 0; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, off, 16));
+      const float scale = fmaxf(__fdiv_rn(amax, 448.f), FLT_MIN);
+      if ((tid & 15) == 0) reinterpret_cast<float*>(crow8 + 512)[tid >> 4] = scale;
+      uint8_t o[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[j] = __nv_cvt_float_to_fp8(__fdiv_rn(bf(h[j]), scale), __NV_SATFINITE, __NV_E4M3);
+      *reinterpret_cast<uint2*>(crow8 + tid * 8) = *reinterpret_cast<const uint2*>(o);
+    }
+  } else if (slot >= 0) {
     const __nv_bfloat16* src = kv_c + (size_t)t * 512;
     for (int i = tid; i < 512 / 8; i += 128) {
       const uint4 v = *reinterpret_cast<const uint4*>(src + i * 8);
@@ -232,7 +257,7 @@ extern "C" {
 int b200_mla_rope_cache_write(void* stream, void* q_pe, void* k_pe, const void* kv_c, const int64_t* positions,
                               const void* cos_sin_cache, int is_neox, const int64_t* slot_mapping, void* kv_cache,
                               int kv_dtype, float kv_scale, int num_tokens, int num_heads) {
-  if (!q_pe || !k_pe || !kv_c || !positions || !cos_sin_cache || !kv_cache || num_heads <= 0 || kv_dtype < 0 || kv_dtype > 1 ||
+  if (!q_pe || !k_pe || !kv_c || !positions || !cos_sin_cache || !kv_cache || num_heads <= 0 || kv_dtype < 0 || kv_dtype > 2 ||
       !(kv_scale > 0.f)) {
     set_error("b200_mla_rope_cache_write: bad argument");
     return B200_ERR_INVALID;

@@ -161,6 +161,11 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
                   const int32_t* page_table, int batch, int q_len, int Hq, int page_size, int max_pages, float sm_scale,
                   int num_splits, float* part_o, float* part_ml, int kv_fp8 = 0, int q_fp8 = 0, float descale_q = 1.f,
                   float descale_k = 1.f);
+// sparse MLA decode (attention over each query token's top-k keys); kv_ds_mla: 656-byte fp8_ds_mla rows, else bf16
+int launch_mla_sparse_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const void* kv, int kv_ds_mla,
+                         const int32_t* topk_idx, int topk, const int32_t* req_id, const int32_t* page_table, int max_pages,
+                         int num_tokens, int Hq, int page_size, float sm_scale, int num_splits, float* part_o,
+                         float* part_ml);
 // split merge of the MLA partials fused with the v up-projection (mla_aux.cu), over rows (b * q_len + i, h)
 void launch_mla_merge_vup(cudaStream_t st, const float* part_o, const float* part_ml, int rows, int num_splits, int Hq,
                           const void* w_uv, void* out_v, void* out_latent, float* lse);

@@ -235,20 +235,73 @@ def mla_decode(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_c_and_k_pe_cache: to
     return out, lse
 
 
+def mla_decode_sparse(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_cache: torch.Tensor, topk_indices: torch.Tensor,
+                      req_id: torch.Tensor, page_table: torch.Tensor, sm_scale: float, num_kv_splits: int = 0,
+                      w_uv: torch.Tensor | None = None):
+    """Sparse MLA decode of DeepSeek-V3.2 / GLM-5 layers (config.index_topk): query token t attends only to the keys
+    topk_indices[t] its lightning indexer picked (request-local positions of request req_id[t]; -1, or a position past the
+    page table, is no key).  Replaces the reference's index conversion plus FlashMLA sparse decode
+    (sparse_utils.py:120, flashmla_sparse.py:587-611, 763-830) with one kernel.  q_nope [T,Hq,512] / q_pe [T,Hq,64] bf16;
+    kv_cache bf16 [pages, page, 576] or the fp8_ds_mla cache, uint8 [pages, page, 656]; topk_indices int32 [T, topk];
+    req_id [T]; page_table [R, max_pages].  A token with no valid entry gets out 0 and lse -inf.
+    With ``w_uv`` [Hq,512,128] the split merge is fused with the v up-projection and (out_v [T,Hq,128], out, lse) is
+    returned.  Returns (out bf16 [T,Hq,512], lse f32 [T,Hq])."""
+    qn, qp = _cuda(q_nope, "q_nope"), _cuda(q_pe, "q_pe")
+    kv = _cuda(kv_cache, "kv_cache")
+    if qn.dtype != torch.bfloat16 or qp.dtype != torch.bfloat16:
+        raise ValueError(f"sparse MLA decode takes bf16 queries, got {qn.dtype} / {qp.dtype}")
+    if kv.dim() != 3 or (kv.dtype, kv.shape[-1]) not in ((torch.bfloat16, 576), (torch.uint8, 656)):
+        raise ValueError(f"kv_cache must be bf16 [pages, page, 576] or fp8_ds_mla uint8 [pages, page, 656], "
+                         f"got {kv.dtype} {tuple(kv.shape)}")
+    T, Hq, _ = qn.shape
+    idx = _cuda(topk_indices.to(torch.int32), "topk_indices")
+    rid = _cuda(req_id.reshape(-1).to(torch.int32), "req_id")
+    pt = _cuda(page_table.to(torch.int32), "page_table")
+    if idx.dim() != 2 or idx.shape[0] != T or rid.numel() != T or qp.shape[0] != T:
+        raise ValueError(f"q_pe, topk_indices and req_id need one row per query token ({T})")
+    if pt.dim() != 2:
+        raise ValueError(f"page_table must be [requests, max_pages], got {tuple(pt.shape)}")
+    topk = idx.shape[1]
+    if num_kv_splits <= 0:
+        # as ops.mla_decode: a CTA = (token, split, value-dim quarter) walks ceil(tiles / splits) 128-entry index tiles;
+        # enough splits to fill ~2 waves of the 132 SMs
+        tiles = -(-topk // 128)
+        num_kv_splits = max(1, min(tiles, 264 // (4 * T)))
+    ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(T, Hq, num_kv_splits), dtype=torch.uint8, device=qn.device)
+    out = torch.empty(T, Hq, 512, dtype=torch.bfloat16, device=qn.device)
+    lse = torch.empty(T, Hq, dtype=torch.float32, device=qn.device)
+    args = [_stream(), qn.data_ptr(), qp.data_ptr(), kv.data_ptr(), 2 if kv.dtype == torch.uint8 else 0, idx.data_ptr(), topk,
+            rid.data_ptr(), pt.data_ptr(), pt.shape[1], T, Hq, kv.shape[1], float(sm_scale), num_kv_splits, ws.data_ptr(),
+            out.data_ptr(), lse.data_ptr()]
+    if w_uv is not None:
+        wv = _cuda(w_uv, "w_uv")
+        assert wv.dtype == torch.bfloat16 and wv.shape == (Hq, 512, 128)
+        out_v = torch.empty(T, Hq, 128, dtype=torch.bfloat16, device=qn.device)
+        L.check(L.lib().b200_mla_decode_sparse(*args, wv.data_ptr(), out_v.data_ptr()), "b200_mla_decode_sparse")
+        return out_v, out, lse
+    L.check(L.lib().b200_mla_decode_sparse(*args, None, None), "b200_mla_decode_sparse")
+    return out, lse
+
+
 def mla_rope_cache_write(q_pe: torch.Tensor, k_pe: torch.Tensor, kv_c: torch.Tensor, positions: torch.Tensor,
                          cos_sin_cache: torch.Tensor, slot_mapping: torch.Tensor, kv_cache: torch.Tensor,
                          is_neox_style: bool = False, kv_scale: float = 1.0) -> None:
     """RoPE of q_pe [T,Hq,64] / k_pe [T,64] IN PLACE (reference RotaryEmbedding.forward_static) fused with
-    concat_and_cache_mla: kv_cache [blocks, block_size, 576] (bf16 or e4m3) row slot_mapping[t] <- [kv_c[t] | rope(k_pe[t])]."""
+    concat_and_cache_mla: kv_cache [blocks, block_size, 576] (bf16 or e4m3) row slot_mapping[t] <- [kv_c[t] | rope(k_pe[t])].
+    A uint8 [blocks, block_size, 656] cache is the fp8_ds_mla layout of concat_and_cache_ds_mla_kernel (per-128-dim fp32
+    scales, bf16 rope part; kv_scale is not used)."""
     for t, n in ((q_pe, "q_pe"), (k_pe, "k_pe"), (kv_c, "kv_c"), (cos_sin_cache, "cos_sin_cache")):
         assert t.is_cuda and t.is_contiguous() and t.dtype == torch.bfloat16, n
-    assert kv_cache.is_cuda and kv_cache.is_contiguous() and kv_cache.shape[-1] == 576 and cos_sin_cache.shape[-1] == 64
+    ds_mla = kv_cache.dtype == torch.uint8 and kv_cache.shape[-1] == 656
+    assert kv_cache.is_cuda and kv_cache.is_contiguous() and (ds_mla or kv_cache.shape[-1] == 576)
+    assert cos_sin_cache.shape[-1] == 64
     T, Hq, _ = q_pe.shape
     pos = _cuda(positions.to(torch.int64), "positions")
     sm = _cuda(slot_mapping.to(torch.int64), "slot_mapping")
     rc = L.lib().b200_mla_rope_cache_write(_stream(), q_pe.data_ptr(), k_pe.data_ptr(), kv_c.data_ptr(), pos.data_ptr(),
                                            cos_sin_cache.data_ptr(), int(is_neox_style), sm.data_ptr(), kv_cache.data_ptr(),
-                                           int(kv_cache.dtype == torch.float8_e4m3fn), float(kv_scale), T, Hq)
+                                           2 if ds_mla else int(kv_cache.dtype == torch.float8_e4m3fn), float(kv_scale),
+                                           T, Hq)
     L.check(rc, "b200_mla_rope_cache_write")
 
 
