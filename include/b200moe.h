@@ -245,6 +245,45 @@ int b200_mla_decode_vup(void* stream, const void* q_nope, const void* q_pe, int 
                         float descale_q, float descale_k, const int32_t* seq_lens, const int32_t* page_table, int batch,
                         int num_heads, int page_size, int max_pages, float sm_scale, int num_splits, void* workspace,
                         const void* w_uv, void* out_v, void* out_latent, float* lse);
+/* The lightning indexer of DeepSeek-V3.2 / GLM-5 layers for decode: it produces the topk_indices that
+ * b200_mla_decode_sparse takes.  Index heads H, head dim 128 = [64 rotary | 64 nope].  The indexer cache is uint8
+ * [num_blocks, block_size, 132] (indexer_k_quant_and_cache's layout): block b holds block_size x 128 e4m3 bytes, then
+ * block_size fp32 scales, one per token.  It shares the latent cache's page table.  All three are CUDA-graph capturable:
+ * no allocation, no synchronisation; a bad shape or misaligned pointer returns B200_ERR_INVALID and launches nothing.
+ *
+ *  b200_indexer_qk_rope_quant_cache_write  replaces the reference's _fused_indexer_q_rope_quant_kernel
+ *      (sparse_attn_indexer.py:127-251), the RoPE of the indexer k (RotaryEmbedding.forward_static) and
+ *      indexer_k_quant_and_cache (csrc/libtorch_stable/cache_kernels.cu:599-659), in one launch.
+ *      q [T,H,128] bf16 contiguous (wq_b output), weights bf16 [T, >= H] with row stride weights_row_stride elements (a
+ *      column slice of the fused projection), k [T,128] bf16 (after k_norm), positions i64 [T] (clamped to the table),
+ *      cos_sin_cache bf16 [max_position, 64] = cos | sin, is_neox 1 = NeoX halves, 0 = interleaved pairs.
+ *      q: RoPE in fp32 (products and sum rounded separately, no FMA), each rotated value rounded to bf16; q_scale = the power of two >= max(amax, 1e-10) / 448 over the
+ *      128 dims; q_fp8 [T,H,128] = e4m3(q / q_scale); weights_out f32 [T,H] = weight * q_scale * softmax_scale * head_scale.
+ *      k: RoPE in bf16 arithmetic; scale = max(amax, 1e-4) / 448 (its power-of-two ceiling when use_ue8m0); row
+ *      slot_mapping[t] (< 0: nothing written) <- e4m3(k / scale) and the fp32 scale.
+ *      1 <= num_heads <= 128; q, k, q_fp8, k_cache 16-byte aligned.
+ *  b200_indexer_logits  replaces DeepGEMM fp8_fp4_paged_mqa_logits (fp8_paged_mqa_logits_torch,
+ *      rocm_aiter_mla_sparse.py:264-363).  q_fp8 [B*Q,H,128] e4m3, weights f32 [B*Q,H] (weights_out above), seq_lens i32 [B]
+ *      (<= max_pages * page_size), page_table i32 [B, max_pages], k_cache with num_blocks blocks of page_size rows.
+ *      logits f32 [B*Q, logits_stride], logits_stride >= max_pages * page_size: row r = b*Q + i,
+ *      logits[r, j] = k_scale[j] * sum_h weights[r, h] * relu(q_fp8[r, h] . k[j]) for j < row_end = S_b - Q + i + 1 (the
+ *      end-aligned causal mask); -inf from row_end to the end of request b's last page; nothing else is written.
+ *      num_heads 32 or 64, 1 <= q_len <= 16, page_size 16, 32 or 64.
+ *  b200_indexer_topk  replaces top_k_per_row_decode (csrc/libtorch_stable/sampler.cu:567-614, 661-720).  Row r of the
+ *      logits starts at r * logits_stride and holds row_width <= logits_stride values.  For row r = b*Q + i with
+ *      row_end = min(max(0, S_b - Q + i + 1), row_width): out i32 [B*Q, topk] = the positions of the
+ *      topk largest logits of [0, row_end) in ascending order, ties at the threshold to the lowest positions; row_end <=
+ *      topk gives 0 .. row_end - 1; -1 pads.  The same bits on every call.  1 <= topk <= 2048. */
+int b200_indexer_qk_rope_quant_cache_write(void* stream, const void* q, const void* weights, int64_t weights_row_stride,
+                                           const void* k, const int64_t* positions, const void* cos_sin_cache,
+                                           int max_position, int is_neox, const int64_t* slot_mapping, void* k_cache,
+                                           int block_size, int use_ue8m0, float softmax_scale, float head_scale,
+                                           void* q_fp8, float* weights_out, int num_tokens, int num_heads);
+int b200_indexer_logits(void* stream, const void* q_fp8, const float* weights, const void* k_cache, int num_blocks,
+                        int page_size, const int32_t* seq_lens, const int32_t* page_table, int batch, int q_len,
+                        int num_heads, int max_pages, float* logits, int64_t logits_stride);
+int b200_indexer_topk(void* stream, const float* logits, int64_t logits_stride, int64_t row_width, const int32_t* seq_lens,
+                      int batch, int q_len, int topk, int32_t* out);
 /* Paged GQA decode.  q [B,Hq,D] bf16, k_cache/v_cache [num_pages,page_size,Hkv,D] bf16 (contiguous), D=128;
  * out bf16 [B,Hq,D], lse f32 [B,Hq] or NULL. */
 int64_t b200_gqa_decode_workspace_bytes(int batch, int num_q_heads, int head_dim, int num_splits);

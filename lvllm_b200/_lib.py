@@ -70,6 +70,10 @@ PROTOTYPES = {
     "b200_mla_q_absorb": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32]),
     "b200_mla_decode_vup": (_i32, [_vp, _vp, _vp, _i32, _vp, _i32, _f32, _f32, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _i32,
                                    _vp, _vp, _vp, _vp, _vp]),
+    "b200_indexer_qk_rope_quant_cache_write": (_i32, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _i32,
+                                                      _f32, _f32, _vp, _vp, _i32, _i32]),
+    "b200_indexer_logits": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i64]),
+    "b200_indexer_topk": (_i32, [_vp, _vp, _i64, _i64, _vp, _i32, _i32, _i32, _vp]),
     "b200_gqa_decode_workspace_bytes": (_i64, [_i32, _i32, _i32, _i32]),
     "b200_gqa_decode": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _f32, _i32,
                                _vp, _vp, _vp]),

@@ -115,7 +115,8 @@ __global__ void __launch_bounds__(WARPS * 32)
       for (int i = 0; i < NV; ++i) o[i] *= corr;
 #pragma unroll
       for (int tt = 0; tt < ATT_TOK; ++tt) {
-        const float p = (tt < nt) ? exp2f(sc[tt] - mt) : 0.f;
+        if (tt >= nt) break;   // rows past the tile's tokens hold stale shared memory: 0 * NaN would poison o
+        const float p = exp2f(sc[tt] - mt);
         l += p;
 #pragma unroll
         for (int i = 0; i < NV; ++i) o[i] = fmaf(p, __bfloat162float(vs[tt][lane + 32 * i]), o[i]);

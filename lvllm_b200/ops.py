@@ -419,3 +419,113 @@ def gqa_qknorm_rope_cache_write(qkv: torch.Tensor, positions: torch.Tensor, cos_
         q_out.data_ptr(), T, num_heads, num_kv_heads, 128)
     L.check(rc, "b200_gqa_qknorm_rope_cache_write")
     return q_out
+
+
+def indexer_qk_rope_quant_cache_write(q: torch.Tensor, weights: torch.Tensor, k: torch.Tensor, positions: torch.Tensor,
+                                      cos_sin_cache: torch.Tensor, slot_mapping: torch.Tensor, k_cache: torch.Tensor,
+                                      softmax_scale: float, head_scale: float, is_neox_style: bool = True,
+                                      use_ue8m0: bool = True):
+    """The lightning indexer's q / k preparation in one launch (reference _fused_indexer_q_rope_quant_kernel,
+    sparse_attn_indexer.py:127-251; RotaryEmbedding.forward_static of k; indexer_k_quant_and_cache,
+    cache_kernels.cu:599-659).  q [T,H,128] bf16 (wq_b output, first 64 dims rotary); weights bf16 [T,H], any row stride
+    (a column slice of the fused projection); k [T,128] bf16 after k_norm; cos_sin_cache bf16 [max_position, 64];
+    slot_mapping [T] (< 0: nothing written); k_cache uint8 [num_blocks, block_size, 132], written in place.
+    Returns (q_fp8 e4m3 [T,H,128], weights_out f32 [T,H] = weight * q_scale * softmax_scale * head_scale)."""
+    x = _cuda(q, "q")
+    kk = _cuda(k, "k")
+    if x.dtype != torch.bfloat16 or x.dim() != 3 or x.shape[2] != 128:
+        raise ValueError(f"q must be bf16 [T, H, 128], got {x.dtype} {tuple(x.shape)}")
+    T, H, _ = x.shape
+    if kk.dtype != torch.bfloat16 or kk.shape != (T, 128):
+        raise ValueError(f"k must be bf16 [{T}, 128], got {kk.dtype} {tuple(kk.shape)}")
+    if not weights.is_cuda or weights.dtype != torch.bfloat16 or weights.shape != (T, H) or weights.stride(1) != 1 \
+            or (T > 1 and weights.stride(0) < H):
+        raise ValueError(f"weights must be a bf16 [{T}, {H}] view with contiguous, non-overlapping rows")
+    cs = _cuda(cos_sin_cache, "cos_sin_cache")
+    if cs.dtype != torch.bfloat16 or cs.dim() != 2 or cs.shape[1] != 64:
+        raise ValueError("cos_sin_cache must be bf16 [max_position, 64]")
+    if not k_cache.is_cuda or k_cache.dtype != torch.uint8 or k_cache.dim() != 3 or k_cache.shape[2] != 132 \
+            or not k_cache.is_contiguous():
+        raise ValueError(f"k_cache must be a contiguous uint8 [num_blocks, block_size, 132], got {tuple(k_cache.shape)}")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    sm = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
+    if pos.numel() != T or sm.numel() != T:
+        raise ValueError("positions and slot_mapping need one entry per token")
+    q_fp8 = torch.empty(T, H, 128, dtype=torch.float8_e4m3fn, device=x.device)
+    w_out = torch.empty(T, H, dtype=torch.float32, device=x.device)
+    rc = L.lib().b200_indexer_qk_rope_quant_cache_write(
+        _stream(), x.data_ptr(), weights.data_ptr(), weights.stride(0) if T > 1 else H, kk.data_ptr(), pos.data_ptr(),
+        cs.data_ptr(), cs.shape[0], int(is_neox_style), sm.data_ptr(), k_cache.data_ptr(), k_cache.shape[1],
+        int(use_ue8m0), float(softmax_scale), float(head_scale), q_fp8.data_ptr(), w_out.data_ptr(), T, H)
+    L.check(rc, "b200_indexer_qk_rope_quant_cache_write")
+    return q_fp8, w_out
+
+
+def _indexer_cache(k_cache: torch.Tensor) -> torch.Tensor:
+    if not k_cache.is_cuda or k_cache.dtype != torch.uint8 or k_cache.dim() != 3 or k_cache.shape[2] != 132 \
+            or not k_cache.is_contiguous():
+        raise ValueError(f"k_cache must be a contiguous uint8 [num_blocks, block_size, 132], got {tuple(k_cache.shape)}")
+    return k_cache
+
+
+def indexer_logits(q_fp8: torch.Tensor, weights: torch.Tensor, k_cache: torch.Tensor, seq_lens: torch.Tensor,
+                   page_table: torch.Tensor, q_len: int = 1, logits: torch.Tensor | None = None) -> torch.Tensor:
+    """Paged MQA logits of the indexer (DeepGEMM fp8_fp4_paged_mqa_logits; fp8_paged_mqa_logits_torch,
+    rocm_aiter_mla_sparse.py:264-363): logits[b*Q + i, j] = k_scale[j] * sum_h weights[b*Q + i, h] * relu(q . k_j) for
+    j <= seq_lens[b] - Q + i; -inf to the end of the request's last page, the rest untouched.  q_fp8 [B*Q,H,128] e4m3,
+    weights f32 [B*Q,H]; H 32 or 64, Q <= 16, page 16 / 32 / 64.  ``logits`` (f32 [B*Q, >= max_pages * page]) is filled
+    in place when given.  Returns logits."""
+    q8 = _cuda(q_fp8, "q_fp8")
+    w = _cuda(weights, "weights")
+    kc = _indexer_cache(k_cache)
+    if q8.dtype != torch.float8_e4m3fn or q8.dim() != 3 or q8.shape[2] != 128:
+        raise ValueError(f"q_fp8 must be e4m3 [B*Q, H, 128], got {q8.dtype} {tuple(q8.shape)}")
+    R, H, _ = q8.shape
+    if w.dtype != torch.float32 or w.shape != (R, H):
+        raise ValueError(f"weights must be f32 [{R}, {H}]")
+    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
+    pt = _cuda(page_table.to(torch.int32), "page_table")
+    B, Q = sl.numel(), int(q_len)
+    if R != B * Q or pt.dim() != 2 or pt.shape[0] < B:
+        raise ValueError(f"q_fp8 needs q_len = {Q} rows per request ({B * Q}), page_table a row per request")
+    page = kc.shape[1]
+    width = pt.shape[1] * page
+    if logits is None:
+        logits = torch.empty(R, width, dtype=torch.float32, device=q8.device)
+    elif logits.dtype != torch.float32 or logits.dim() != 2 or logits.shape[0] != R or logits.shape[1] < width \
+            or logits.stride(1) != 1:
+        raise ValueError(f"logits must be f32 [{R}, >= {width}] with contiguous rows")
+    rc = L.lib().b200_indexer_logits(_stream(), q8.data_ptr(), w.data_ptr(), kc.data_ptr(), kc.shape[0], page,
+                                     sl.data_ptr(), pt.data_ptr(), B, Q, H, pt.shape[1], logits.data_ptr(),
+                                     logits.stride(0))
+    L.check(rc, "b200_indexer_logits")
+    return logits
+
+
+def indexer_topk(logits: torch.Tensor, seq_lens: torch.Tensor, topk: int, q_len: int = 1) -> torch.Tensor:
+    """top_k_per_row_decode (sampler.cu:567-614, 661-720): for row b*Q + i, the positions of the topk largest logits of
+    [0, min(seq_lens[b] - Q + i + 1, logits.shape[1])) in ascending order, ties at the threshold to the lowest positions,
+    -1 padding.  ``logits`` may be a column slice of a wider buffer (rows read through its own row stride).
+    Returns int32 [B*Q, topk]."""
+    lg = logits
+    if not lg.is_cuda or lg.dtype != torch.float32 or lg.dim() != 2 or lg.stride(1) != 1 \
+            or (lg.shape[0] > 1 and lg.stride(0) < lg.shape[1]):
+        raise ValueError("logits must be a CUDA f32 [rows, width] tensor with contiguous, non-overlapping rows")
+    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
+    B, Q = sl.numel(), int(q_len)
+    if lg.shape[0] != B * Q:
+        raise ValueError(f"logits needs q_len = {Q} rows per request ({B * Q}), got {lg.shape[0]}")
+    out = torch.empty(B * Q, int(topk), dtype=torch.int32, device=lg.device)
+    row_stride = lg.stride(0) if lg.shape[0] > 1 else lg.shape[1]
+    rc = L.lib().b200_indexer_topk(_stream(), lg.data_ptr(), row_stride, lg.shape[1], sl.data_ptr(), B, Q, int(topk),
+                                   out.data_ptr())
+    L.check(rc, "b200_indexer_topk")
+    return out
+
+
+def indexer_decode(q_fp8: torch.Tensor, weights: torch.Tensor, k_cache: torch.Tensor, seq_lens: torch.Tensor,
+                   page_table: torch.Tensor, q_len: int, topk: int) -> torch.Tensor:
+    """The indexer's decode step: indexer_logits then indexer_topk.  Returns topk_indices int32 [B*Q, topk], request-local
+    positions, the layout mla_decode_sparse takes with req_id = row // q_len and the same page table."""
+    logits = indexer_logits(q_fp8, weights, k_cache, seq_lens, page_table, q_len)
+    return indexer_topk(logits, seq_lens, topk, q_len)
