@@ -14,10 +14,14 @@
 //   L[128, N]           = 1[128, 128 tokens] . P^T                 (row sums of P on the tensor core: every
 //                                                                   epilogue thread reads l[h] from its own lane)
 // K and V tiles are gathered with cp.async straight into 128B-swizzled [64-dim block][128 tokens][128 B] blocks; a row is
-// found through (page, slot, head) strides, so the K / V halves of a packed NHD / HND cache are read in place;
-// NST stages of (Q, K, V) let the loaders run ahead of the MMAs; the accumulators cross from the MMA warpgroup to the
-// softmax / epilogue threads through the exchange area (common.cuh), S^T double-buffered so that QK^T of item n+1
-// overlaps softmax of item n.  Partial (O, m, l) per split are merged by attn_merge_kernel.
+// found through (page, slot, head) strides, so the K / V halves of a packed NHD / HND cache are read in place.
+// Two rings let the loaders run ahead of the MMAs: NK stages of (Q, K), each freed as soon as QK^T of its item has
+// completed, and NV stages of V, each freed after PV of its item (which waits for the item's softmax).  Splitting them
+// keeps K from sitting in shared memory through the softmax, so the freed space carries the next item's K early.  The
+// accumulators cross from the MMA warpgroup to the softmax / epilogue threads through the exchange area (common.cuh),
+// S^T double-buffered so that QK^T of item n+1 overlaps softmax of item n.  Softmax and epilogue stop at the item's
+// real columns (ncols <= N, in runs of 4); the P tiles are zeroed once, so the columns they skip feed PV finite values
+// that reach only O / L columns nobody reads.  Partial (O, m, l) per split are merged by attn_merge_kernel.
 // Reference semantics: tests/kernels/attention/test_flashinfer.py:29-80 (ref_paged_attn, decode case).
 // Roofline: HBM — algorithmic bytes = sum_b S_b * Hkv * 128 * 2 (K and V) * 2 B * n_qg (n_qg = ceil(Q / Qg) q-groups).
 #include <math_constants.h>
@@ -30,14 +34,16 @@ namespace b200 {
 
 constexpr int GQA_TOK = 128;
 constexpr int GQA_THREADS = 512;          // warps 0-3 / 4-7: softmax+epilogue groups, 8-11 loaders, 12-15 MMA warpgroup
-constexpr int GQA_MAX_STAGES = 3;
+constexpr int GQA_MAX_STAGES = 3;         // per ring
+constexpr int GQA_MIN_STAGES = 2;         // per ring: the MMA warpgroup issues QK of item n + 1 before PV of item n
+constexpr int GQA_V_STAGES = 2;           // V stages: the rest of shared memory goes to (Q, K) stages
 constexpr int GQA_SMEM_MAX = 232448;
 constexpr int GQA_MAX_ITEMS = 1024;       // items per CTA the token-count table holds
-constexpr int GQA_MAX_N = 32;             // query heads per kv head (rounded up to 16) that leave two pipeline stages: the exchange area
-                                          // (512 B per head and group), the P tiles and a 64 KB + Q stage grow with it
+constexpr int GQA_MAX_N = 32;             // query heads per kv head (rounded up to 16) that leave two stages per ring: the exchange area
+                                          // (512 B per head and group), the P tiles and the Q rows of a (Q, K) stage grow with it
 
 struct GqaBars {
-  uint64_t qk_full[GQA_MAX_STAGES], v_full[GQA_MAX_STAGES], kv_free[GQA_MAX_STAGES];
+  uint64_t qk_full[GQA_MAX_STAGES], k_free[GQA_MAX_STAGES], v_full[GQA_MAX_STAGES], v_free[GQA_MAX_STAGES];
   uint64_t s_full[2], p_full[2], o_full[2], o_done[2];
   float lsum[2][GQA_MAX_N];        // row sums of P per head (the rows of L are all the same: one is kept)
   alignas(16) float wmax[2][4][GQA_MAX_N];
@@ -65,7 +71,7 @@ B200_DEVICE void bar_sync_group(int g) { asm volatile("bar.sync %0, 128;" ::"r"(
 
 // SPEC: Q > 1 query tokens per request.  Without it every q-group expression below is a compile-time constant (Q = Qg = 1,
 // columns = heads), which keeps the single-token decode free of the per-column bookkeeping.
-// smem: [ones 1 KB][P group 0 | P group 1: 2 x N x 128 B each][stage: Q (2 x N x 128 B) | K 32 KB | V 32 KB] x NST
+// smem: [ones 1 KB][P group 0 | P group 1: 2 x N x 128 B each][(Q (2 x N x 128 B) | K 32 KB) x NK][V 32 KB x NV]
 //       [exchange: 2 groups x N columns x 512 B][bars]
 template <int N, bool SPEC>
 __global__ void __launch_bounds__(GQA_THREADS, 1)
@@ -73,17 +79,18 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
                          const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ seq_lens,
                          int64_t block_stride, int64_t page_stride, int64_t head_stride,
                          const int32_t* __restrict__ page_table, int B, int Hq, int Hkv, int page_size, int max_pages,
-                         float scale_log2, int num_splits, int Q_, int Qg_, int NST, float* __restrict__ part_o,
+                         float scale_log2, int num_splits, int Q_, int Qg_, int NK, int NV, float* __restrict__ part_o,
                          float* __restrict__ part_ml) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int qbytes = N * 128;                       // one 64-dim block of the Q (or P) rows
   const int pbytes = (2 * qbytes + 1023) & ~1023;   // one group's P tile
-  const int stage_bytes = 2 * qbytes + 4 * TILE_BYTES;
+  const int kstage_bytes = 2 * qbytes + 2 * TILE_BYTES;
   uint8_t* ones = smem;
   uint8_t* p_base = smem + 1024;
-  uint8_t* stages = p_base + 2 * pbytes;
-  uint8_t* xch_area = stages + (size_t)NST * stage_bytes;
+  uint8_t* kstages = p_base + 2 * pbytes;
+  uint8_t* vstages = kstages + (size_t)NK * kstage_bytes;
+  uint8_t* xch_area = vstages + (size_t)NV * 2 * TILE_BYTES;
   GqaBars* bars = reinterpret_cast<GqaBars*>(xch_area + 2 * N * 512);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int G = Hq / Hkv;
@@ -96,8 +103,9 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
   if (tid == 0) {
     for (int i = 0; i < GQA_MAX_STAGES; ++i) {
       mbar_init(&bars->qk_full[i], 128);
+      mbar_init(&bars->k_free[i], 1);
       mbar_init(&bars->v_full[i], 128);
-      mbar_init(&bars->kv_free[i], 1);
+      mbar_init(&bars->v_free[i], 1);
     }
     for (int g = 0; g < 2; ++g) {
       mbar_init(&bars->s_full[g], 128);   // every MMA thread, after parking its fragment
@@ -119,6 +127,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
   if (SPEC && tid < GQA_MAX_N) bars->col_row[tid] = (tid / G) * Hq + tid % G;
   auto col_row = [&](int c) { return SPEC ? bars->col_row[c] : c; };
   if (tid < 64) reinterpret_cast<uint4*>(ones)[tid] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
+  for (int i = tid; i < 2 * pbytes / 16; i += GQA_THREADS) reinterpret_cast<uint4*>(p_base)[i] = make_uint4(0u, 0u, 0u, 0u);
   fence_proxy_async();
   __syncthreads();
   // group g owns columns [N*g, N*g + N): S^T of an item until its softmax has written P, then O^T of the same item
@@ -150,11 +159,11 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
                   b = rest / (n_qg * Hkv);
         const int ncols = SPEC ? G * min(Qg, Q - qg * Qg) : G;
         const __nv_bfloat16* qrow0 = q + ((size_t)(b * Q + qg * Qg) * Hq + kvh * G) * 128 + c * 8;
-        const int s = n % NST;
-        uint8_t* q_t = stages + (size_t)s * stage_bytes;
+        const int sk = n % NK, sv = n % NV;
+        uint8_t* q_t = kstages + (size_t)sk * kstage_bytes;
         uint8_t* k_t = q_t + 2 * qbytes;
-        uint8_t* v_t = k_t + 2 * TILE_BYTES;
-        gqa_wait(&bars->kv_free[s], ((n / NST) & 1) ^ 1);
+        uint8_t* v_t = vstages + (size_t)sv * 2 * TILE_BYTES;
+        gqa_wait(&bars->k_free[sk], ((n / NK) & 1) ^ 1);
         for (int r = r0; r < N; r += 16) {
           const bool qok = r < ncols;
           const __nv_bfloat16* src = qrow0 + (size_t)(qok ? col_row(r) : 0) * 128;
@@ -175,7 +184,8 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
             cp_async16(k_t + kb * TILE_BYTES + sw128_offset(r0 + 16 * u, c * 16), ok ? kc + rowoff[u] + kb * 64 : kc, ok);
           }
         }
-        cp_async_mbar_arrive_noinc(&bars->qk_full[s]);
+        cp_async_mbar_arrive_noinc(&bars->qk_full[sk]);
+        gqa_wait(&bars->v_free[sv], ((n / NV) & 1) ^ 1);
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb) {
 #pragma unroll
@@ -184,7 +194,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
             cp_async16(v_t + kb * TILE_BYTES + sw128_offset(r0 + 16 * u, c * 16), ok ? vc + rowoff[u] + kb * 64 : vc, ok);
           }
         }
-        cp_async_mbar_arrive_noinc(&bars->v_full[s]);
+        cp_async_mbar_arrive_noinc(&bars->v_full[sv]);
         ++n;
       }
 #pragma unroll
@@ -195,10 +205,10 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
     const bool lead = tid == 12 * 32;
     const uint32_t oa = smem_u32(ones);
     auto issue_qk = [&](uint32_t n) {
-      const int s = n % NST, g = n & 1;
-      gqa_wait(&bars->qk_full[s], (n / NST) & 1);
+      const int s = n % NK, g = n & 1;
+      gqa_wait(&bars->qk_full[s], (n / NK) & 1);
       fence_proxy_async();   // LDGSTS (generic proxy) writes -> wgmma (async proxy) reads
-      const uint32_t qa = smem_u32(stages + (size_t)s * stage_bytes), ka = qa + 2 * qbytes;
+      const uint32_t qa = smem_u32(kstages + (size_t)s * kstage_bytes), ka = qa + 2 * qbytes;
       float sacc[2][N / 2];                                               // A = K (K-major), B = Q (K-major)
       wgmma_fence();
 #pragma unroll
@@ -208,6 +218,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
           wgmma_tile128<N, 1>(sacc, ka + kb * TILE_BYTES + ks * 32, qa + kb * qbytes + ks * 32, (kb > 0 || ks > 0) ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<0>();
+      if (lead) mbar_arrive(&bars->k_free[s]);
       // the columns still hold O^T of the group's previous item until its epilogue has read them (its PV was issued
       // before this QK, so the wait cannot block the MMAs it depends on)
       if (n >= 2) gqa_wait(&bars->o_done[g], ((n >> 1) - 1) & 1);
@@ -216,11 +227,11 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       mbar_arrive(&bars->s_full[g]);
     };
     auto issue_pv = [&](uint32_t n) {
-      const int s = n % NST, g = n & 1;
+      const int s = n % NV, g = n & 1;
       gqa_wait(&bars->p_full[g], (n >> 1) & 1);
-      gqa_wait(&bars->v_full[s], (n / NST) & 1);
+      gqa_wait(&bars->v_full[s], (n / NV) & 1);
       fence_proxy_async();
-      const uint32_t va = smem_u32(stages + (size_t)s * stage_bytes) + 2 * qbytes + 2 * TILE_BYTES;
+      const uint32_t va = smem_u32(vstages + (size_t)s * 2 * TILE_BYTES);
       const uint32_t pa = smem_u32(p_base + g * pbytes);
       float oacc[2][N / 2], lacc[N / 2];   // the rows of L are all the same: one 64-row half serves both
       wgmma_fence();
@@ -235,7 +246,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       }
       wgmma_commit();
       wgmma_wait<0>();
-      if (lead) mbar_arrive(&bars->kv_free[s]);
+      if (lead) mbar_arrive(&bars->v_free[s]);
       // p_full was waited for above: the group's softmax is done with S^T, O^T takes its place
 #pragma unroll
       for (int h = 0; h < 2; ++h) xch_store_frag<N>(tm + g * N, h, oacc[h]);
@@ -290,15 +301,24 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       const bool tv = t < nt;
       gqa_wait(&bars->s_full[g], ph);
       float my_ms = 0.f;                          // thread t == h keeps m[h] * scale for the partial record
-      for (int c0 = 0; c0 < N; c0 += 16) {
+      // columns >= ncols (zero Q rows) are skipped in runs of 4, which keeps 4 columns of shuffles and ex2 in flight
+      // (the columns of a run past ncols compute finite values nobody reads).  ncols is the same for every thread of the
+      // CTA, so the group's barriers stay matched.  The blocks of 16 columns: one at N = 16, a loop of compile-time
+      // length; at N = 32 a loop over the blocks that hold real columns (unrolled over both, it ran slower).
+      const int cend = N == 16 ? 16 : ncols;
+      for (int c0 = 0; c0 < cend; c0 += 16) {
         float v[16];
         __syncwarp();
         xch_ld<16>(tm_s + c0, v);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          v[j] = (SPEC ? c0 + j >= cmin : tv) ? v[j] : -CUDART_INF_F;
-          const float wm = warp_max(v[j]);
-          if (lane == j) wmax[warp & 3][c0 + j] = wm;
+        for (int j4 = 0; j4 < 16; j4 += 4) {
+          if (c0 + j4 >= ncols) break;
+#pragma unroll
+          for (int j = j4; j < j4 + 4; ++j) {
+            v[j] = (SPEC ? c0 + j >= cmin : tv) ? v[j] : -CUDART_INF_F;
+            const float wm = warp_max(v[j]);
+            if (lane == j) wmax[warp & 3][c0 + j] = wm;
+          }
         }
         bar_sync_group(g);
         float m[16];
@@ -315,16 +335,20 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
         }
         uint8_t* pr = prow + (c0 >> 3) * 1024;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float ms = m[j] * scale_log2;
-          my_ms = (t == c0 + j) ? ms : my_ms;
-          // masked tokens: ex2(-inf) = 0; a column with no visible token in this split (m = -inf) gets P = 0, l = 0 and
-          // records m = -inf, which the merge skips
-          const float p = SPEC && m[j] == -CUDART_INF_F ? 0.f : ex2_approx(fmaf(v[j], scale_log2, -ms));
-          *reinterpret_cast<__nv_bfloat16*>(pr + (j >> 3) * 1024 + (j & 7) * 128 + ((bch ^ (j & 7)) << 4) + blo) =
-              __float2bfloat16_rn(p);
+        for (int j4 = 0; j4 < 16; j4 += 4) {
+          if (c0 + j4 >= ncols) break;
+#pragma unroll
+          for (int j = j4; j < j4 + 4; ++j) {
+            const float ms = m[j] * scale_log2;
+            my_ms = (t == c0 + j) ? ms : my_ms;
+            // masked tokens: ex2(-inf) = 0; a column with no visible token in this split (m = -inf) gets P = 0, l = 0
+            // and records m = -inf, which the merge skips
+            const float p = SPEC && m[j] == -CUDART_INF_F ? 0.f : ex2_approx(fmaf(v[j], scale_log2, -ms));
+            *reinterpret_cast<__nv_bfloat16*>(pr + (j >> 3) * 1024 + (j & 7) * 128 + ((bch ^ (j & 7)) << 4) + blo) =
+                __float2bfloat16_rn(p);
+          }
         }
-        if (c0 + 16 < N) bar_sync_group(g);       // wmax is reused by the next 16 heads
+        if (c0 + 16 < ncols) bar_sync_group(g);   // wmax is reused by the next 16 heads
       }
       fence_proxy_async();
       mbar_arrive(&bars->p_full[g]);
@@ -332,7 +356,7 @@ __global__ void __launch_bounds__(GQA_THREADS, 1)
       // epilogue: thread = value dim d, columns = heads
       float* po = part_o + pbase * 128 + t;
       const size_t hstride = (size_t)num_splits * 128;
-      for (int c0 = 0; c0 < N; c0 += 16) {
+      for (int c0 = 0; c0 < cend; c0 += 16) {
         float o[16];
         __syncwarp();
         xch_ld<16>(tm_o + c0, o);
@@ -420,18 +444,19 @@ int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc
   const int qbytes = N * 128;
   const int fixed = 1024 /*align*/ + 1024 /*ones*/ + 2 * ((2 * qbytes + 1023) & ~1023) + 2 * N * 512 /*exchange*/ +
                     (int)sizeof(GqaBars) + 64;
-  const int stage_bytes = 2 * qbytes + 4 * TILE_BYTES;
-  int nst = (GQA_SMEM_MAX - fixed) / stage_bytes;
-  if (nst > GQA_MAX_STAGES) nst = GQA_MAX_STAGES;
-  // the MMA warpgroup issues QK of item n + 1 before PV of item n, which is what frees item n's stage: two stages at least
-  static_assert((GQA_SMEM_MAX - (2048 + 4 * GQA_MAX_N * 128 + 2 * GQA_MAX_N * 512 + (int)sizeof(GqaBars) + 64)) /
-                        (2 * GQA_MAX_N * 128 + 4 * TILE_BYTES) >= 2,
-                "gqa_decode_tc: two pipeline stages at the largest group");
-  if (nst < 2) {
+  const int kstage_bytes = 2 * qbytes + 2 * TILE_BYTES, vstage_bytes = 2 * TILE_BYTES;
+  // GQA_V_STAGES of V (a V stage is held through the softmax of its item), as many (Q, K) stages as the rest holds
+  const int nv = GQA_V_STAGES;
+  const int nk = min(GQA_MAX_STAGES, (GQA_SMEM_MAX - fixed - nv * vstage_bytes) / kstage_bytes);
+  static_assert(GQA_MIN_STAGES <= GQA_V_STAGES && GQA_V_STAGES <= GQA_MAX_STAGES, "gqa_decode_tc: V ring size");
+  static_assert((GQA_SMEM_MAX - (2048 + 4 * GQA_MAX_N * 128 + 2 * GQA_MAX_N * 512 + (int)sizeof(GqaBars) + 64) -
+                 GQA_V_STAGES * 2 * TILE_BYTES) / (2 * GQA_MAX_N * 128 + 2 * TILE_BYTES) >= GQA_MIN_STAGES,
+                "gqa_decode_tc: two (Q, K) stages at the largest group");
+  if (nk < GQA_MIN_STAGES) {
     set_error("gqa_decode_tc: group size does not fit shared memory");
     return B200_ERR_INVALID;
   }
-  const int smem = fixed + nst * stage_bytes;
+  const int smem = fixed + nk * kstage_bytes + nv * vstage_bytes;
   int dev = 0;
   if (const cudaError_t e = cudaGetDevice(&dev); e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
   const int num_sms = device_sms(dev);
@@ -446,7 +471,7 @@ int launch_gqa_tc(cudaStream_t st, const void* q, const void* kc, const void* vc
   kern<<<grid, GQA_THREADS, smem, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(kc),
       reinterpret_cast<const __nv_bfloat16*>(vc), seq_lens, block_stride, page_stride, head_stride, page_table, batch, Hq, Hkv, page_size, max_pages,
-      sm_scale * 1.4426950408889634f, num_splits, q_len, Qg, nst, part_o, part_ml);
+      sm_scale * 1.4426950408889634f, num_splits, q_len, Qg, nk, nv, part_o, part_ml);
   attn_merge_kernel<128><<<batch * q_len * Hq, 32, 0, st>>>(part_o, part_ml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
   g_launches += 2;
   cudaError_t e = cudaGetLastError();
