@@ -29,6 +29,7 @@
 
 #include "common.cuh"
 #include "moe_internal.cuh"
+#include "w4_layout.cuh"
 
 namespace b200 {
 
@@ -89,9 +90,9 @@ struct FCfg {
   static constexpr int MMA_THREADS = WD ? 256 : 128;
   static constexpr int NTHREADS = MMA_WARP0 * 32 + MMA_THREADS;
   // WD: registers after setmaxnreg (consumers / everything else); the pool is the launch's 65536 / NTHREADS rounded
-  // down to 8 per thread.  At 64 columns a consumer holds 64 fp32 accumulators, two slices of A fragments (16) and the
-  // next slice's nibble words (8): below 144 ptxas serialises the wgmmas (C7512).  The narrower instantiations pipeline at
-  // 120 and keep 80 for the other warps.
+  // down to 8 per thread.  At 64 columns a consumer holds 64 fp32 accumulators, two slices of A fragments (16) and two
+  // k-blocks of nibble words and scale records (up to 24): below 144 ptxas serialises the wgmmas (C7512).  The narrower
+  // instantiations pipeline at 120 and keep 80 for the other warps.
   static constexpr int REG_MMA = (WD && TNMAX == 64) ? 144 : 120;
   static constexpr int REG_REST = (WD && TNMAX == 64) ? 64 : 80;
   static_assert(!WD || REG_MMA * MMA_THREADS + REG_REST * (NTHREADS - MMA_THREADS) <= (65536 / NTHREADS) / 8 * 8 * NTHREADS,
@@ -226,101 +227,100 @@ B200_DEVICE void combine_cols(const FusedArgs& a, const FTables* tb, int j, int 
 }
 
 // ------------------------------------------------------------------------------- 4-bit consumer warpgroups
-// A raw [128 x 64] 4-bit tile stores each row's two 32-column halves as four words; word i holds columns 8i..8i+7 in the
-// order the conversion unpacks them (int4: nibbles j and j+4 -> columns 8i+2j, +1; e2m1: byte j -> columns 8i+2j, +1).
-// The wgmma A fragment of a k16 slice wants columns (2t, 2t+1) and (2t+8, 2t+9) of two rows (t = lane % 4): nibble pair /
-// byte t of the slice's two words.  The operation sequence per format is fixed, so the fp16 values are exactly those of
-// the dequantised tile: int4 (1024 + q) - 1032 then * scale; e2m1 bits placed at value * 2^-14, * 2^14, then * scale.
-template <int WQ>
-B200_DEVICE uint32_t w4_pair(uint32_t w, int t, __half2 s2) {
-  __half2 h;
-  if (WQ == 1) {
-    const uint32_t q = ((w >> (4 * t)) & 0x000F000Fu) | 0x64006400u;   // fp16 (1024 + q) pairs
-    h = __hmul2(__hadd2(*reinterpret_cast<const __half2*>(&q), __float2half2_rn(-1032.0f)), s2);   // q - 8 is exact
-  } else {
-    const uint32_t by = (w >> (8 * t)) & 0xFFu;
-    // sign to bit 15, exponent + mantissa to bits [11:9]: value * 2^-14 (the e2m1 subnormal 0.5 lands on an fp16 subnormal)
-    const uint32_t e = ((by & 0x7u) << 9) | ((by & 0x8u) << 12) | ((by & 0x70u) << 21) | ((by & 0x80u) << 24);
-    h = __hmul2(__hmul2(*reinterpret_cast<const __half2*>(&e), __float2half2_rn(16384.0f)), s2);
-  }
-  return *reinterpret_cast<const uint32_t*>(&h);
+// A raw 4-bit tile is stored in the consumers' wgmma fragment order (w4_layout.cuh): per k-block a thread reads its 16
+// nibble bytes and its scale record with one load each, and word ks of the 16 bytes converts to its A fragment of k16
+// slice ks.  The operation sequence per format is fixed, so the fp16 values are exactly those of the dequantised tile:
+// int4 (1024 + q) - 1032, or (1024 + 16q) / 16 - 72, then * scale; e2m1 bits placed at value * 2^-14, * 2^14, then
+// * scale.
+B200_DEVICE uint4 lds_u4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+  return v;
 }
-// scale of row r for the 16 columns [32 grp + 16 sub, +16)
 B200_DEVICE uint2 lds_u2(uint32_t addr) {
   uint2 v;
   asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
   return v;
 }
-B200_DEVICE uint32_t lds_u16(uint32_t addr) {
-  uint16_t v;
-  asm volatile("ld.shared.b16 %0, [%1];" : "=h"(v) : "r"(addr));
-  return v;
-}
-B200_DEVICE uint32_t lds_u8(uint32_t addr) {
+B200_DEVICE uint32_t lds_u32(uint32_t addr) {
   uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
   return v;
 }
-// raw scale of row r for the 16 columns [32 grp + 16 sub, +16) (sc: shared-memory address of the tile's scales) and its
-// conversion to an fp16 pair
-template <int WQ>
-B200_DEVICE uint32_t w4_scale_ld(uint32_t sc, int grp, int sub, int r) {
-  if (WQ == 1) return lds_u16(sc + (grp * 128 + r) * 2);
-  if (WQ == 2) return lds_u8(sc + (2 * grp + sub) * 128 + r);
-  return lds_u8(sc + grp * 128 + r);
+// (a & B) | C in one LOP3: written out, the compiler may emit an AND and an OR
+template <uint32_t B, uint32_t C>
+B200_DEVICE uint32_t and_or(uint32_t a) {
+  uint32_t d;
+  asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(d) : "r"(a), "n"(B), "n"(C));
+  return d;
 }
+B200_DEVICE __half2 u32_h2(uint32_t u) { return *reinterpret_cast<const __half2*>(&u); }
+B200_DEVICE uint32_t h2_u32(__half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
+
+// scales of rows (r0, r0 + 8) for slice ks from the thread's scale record
 template <int WQ>
-B200_DEVICE __half2 w4_scale(uint32_t raw) {
-  if (WQ == 1) {
-    const uint16_t b = (uint16_t)raw;
-    return __half2half2(*reinterpret_cast<const __half*>(&b));
-  }
+B200_DEVICE __half2 w4_scales(uint2 rec, int ks) {
+  if (WQ == 1) return u32_h2(ks < 2 ? rec.x : rec.y);
   if (WQ == 2) {
-    const __half_raw h = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)raw, __NV_E4M3);
-    return __half2half2(*reinterpret_cast<const __half*>(&h));
+    const uint32_t w = ks < 2 ? rec.x : rec.y;
+    const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w >> (16 * (ks & 1))), __NV_E4M3);
+    return *reinterpret_cast<const __half2*>(&h);
   }
   // e8m0 -> fp16 2^(E-127): exponent field E-112 clamped to [0,30] (scales < 2^-14 flush to 0)
-  int f = (int)raw - 112;
-  f = f < 0 ? 0 : (f > 30 ? 30 : f);
-  const uint16_t bits = (uint16_t)(f << 10);
-  return __half2half2(*reinterpret_cast<const __half*>(&bits));
+  const uint32_t w = rec.x >> (16 * (ks >> 1));
+  int f0 = (int)(w & 0xFFu) - 112, f1 = (int)((w >> 8) & 0xFFu) - 112;
+  f0 = f0 < 0 ? 0 : (f0 > 30 ? 30 : f0);
+  f1 = f1 < 0 ? 0 : (f1 > 30 ? 30 : f1);
+  return u32_h2(((uint32_t)f0 << 10) | ((uint32_t)f1 << 26));
+}
+// one nibble word -> the four A fragment registers of one tile (s: scales of rows r0 and r0 + 8)
+template <int WQ>
+B200_DEVICE void w4_frag(uint32_t (&f)[4], uint32_t w, __half2 s) {
+  const __half2 s0 = __low2half2(s), s1 = __high2half2(s);
+  if (WQ == 1) {
+    const __half2 lo_off = __float2half2_rn(-1032.0f), hi_mul = __float2half2_rn(0.0625f), hi_off = __float2half2_rn(-72.0f);
+    const uint32_t l0 = and_or<0x000F000Fu, 0x64006400u>(w), h0 = and_or<0x00F000F0u, 0x64006400u>(w);
+    w >>= 8;
+    const uint32_t l1 = and_or<0x000F000Fu, 0x64006400u>(w), h1 = and_or<0x00F000F0u, 0x64006400u>(w);
+    f[0] = h2_u32(__hmul2(__hadd2(u32_h2(l0), lo_off), s0));            // q - 8 is exact in both forms
+    f[1] = h2_u32(__hmul2(__hfma2(u32_h2(h0), hi_mul, hi_off), s1));
+    f[2] = h2_u32(__hmul2(__hadd2(u32_h2(l1), lo_off), s0));
+    f[3] = h2_u32(__hmul2(__hfma2(u32_h2(h1), hi_mul, hi_off), s1));
+  } else {
+    // sign to bit 15, exponent + mantissa to bits [11:9]: value * 2^-14 (the e2m1 subnormal 0.5 lands on an fp16 subnormal)
+    const uint32_t e[4] = {w & 0x8E008E00u, (w << 3) & 0x8E008E00u, ((w << 9) & 0x0E000E00u) | ((w << 2) & 0x80008000u),
+                           ((w << 6) & 0x0E000E00u) | ((w << 1) & 0x80008000u)};
+    const __half2 p14 = __float2half2_rn(16384.0f);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) f[i] = h2_u32(__hmul2(__hmul2(u32_h2(e[i]), p14), (i & 1) ? s1 : s0));
+  }
 }
 
-// The shared-memory words one thread needs for a k16 slice: rows r0 and r0 + 8 of the gate (na = 0) and up (na = 1) tile.
-// They are loaded one slice ahead, so that their load latency is hidden behind the conversion of the previous slice.  SC:
-// the scales are loaded ahead too.  At 64 columns the accumulators leave no registers for them, and they are loaded with
-// the conversion instead, whose nibble arithmetic covers part of their latency.
-struct W4Slice {
-  uint2 q0[2], q1[2];
-  uint32_t s0[2], s1[2];
+// One thread's shared-memory words of one k-block: the gate (na = 0) and up (na = 1) tiles' 16 nibble bytes and scale
+// records (mxfp4: .x only)
+struct W4Block {
+  uint4 q[2];
+  uint2 s[2];
 };
-template <int WQ, bool SC>
-B200_DEVICE void w4_load(W4Slice& v, uint32_t raw, int tile_bytes, int kk, int ks, int r0) {
-  const int grp = ks >> 1, sub = ks & 1;
+template <int WQ>
+B200_DEVICE void w4_load(W4Block& b, uint32_t raw, int tile_bytes, int kk, uint32_t u) {
 #pragma unroll
   for (int na = 0; na < 2; ++na) {
     const uint32_t tile = raw + (kk * 2 + na) * tile_bytes;
-    v.q0[na] = lds_u2(tile + (grp * 128 + r0) * 16 + sub * 8);
-    v.q1[na] = lds_u2(tile + (grp * 128 + r0 + 8) * 16 + sub * 8);
-    if (SC) {
-      v.s0[na] = w4_scale_ld<WQ>(tile + 4096, grp, sub, r0);
-      v.s1[na] = w4_scale_ld<WQ>(tile + 4096, grp, sub, r0 + 8);
-    }
+    b.q[na] = lds_u4(tile + u * 16);
+    const uint32_t rec = tile + W4_NIBBLE_BYTES + (u >> 2) * w4_scale_record_bytes(WQ);
+    if (WQ == 3)
+      b.s[na] = make_uint2(lds_u32(rec), 0u);
+    else
+      b.s[na] = lds_u2(rec);
   }
 }
-template <int WQ, bool SC>
-B200_DEVICE void w4_convert(uint32_t (&f)[2][4], const W4Slice& v, uint32_t raw, int tile_bytes, int kk, int ks, int r0,
-                            int t) {
-  const int grp = ks >> 1, sub = ks & 1;
+template <int WQ>
+B200_DEVICE void w4_convert(uint32_t (&f)[2][4], const W4Block& b, int ks) {
 #pragma unroll
   for (int na = 0; na < 2; ++na) {
-    const uint32_t sc = raw + (kk * 2 + na) * tile_bytes + 4096;
-    const __half2 s0 = w4_scale<WQ>(SC ? v.s0[na] : w4_scale_ld<WQ>(sc, grp, sub, r0));
-    const __half2 s1 = w4_scale<WQ>(SC ? v.s1[na] : w4_scale_ld<WQ>(sc, grp, sub, r0 + 8));
-    f[na][0] = w4_pair<WQ>(v.q0[na].x, t, s0);
-    f[na][1] = w4_pair<WQ>(v.q1[na].x, t, s1);
-    f[na][2] = w4_pair<WQ>(v.q0[na].y, t, s0);
-    f[na][3] = w4_pair<WQ>(v.q1[na].y, t, s1);
+    const uint32_t w = ks == 0 ? b.q[na].x : ks == 1 ? b.q[na].y : ks == 2 ? b.q[na].z : b.q[na].w;
+    w4_frag<WQ>(f[na], w, w4_scales<WQ>(b.s[na], ks));
   }
 }
 
@@ -341,19 +341,19 @@ B200_DEVICE void frag_hold(uint32_t (&f)[2][4]) {
     for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(f[na][i]));
 }
 
-// k-iterations [ki0, ki1) of one tile at NN token columns: per k16 slice, convert the gate and up fragments of this
-// warpgroup's rows, then issue their two MMAs (A registers, B = token tile of the stage).  Two slices are in flight: the
-// conversion of slice n runs while the MMAs of slice n - 1 execute (wait_group 1), with the shared-memory words of slice
-// n + 1 already requested.  A stage is released once the MMAs of the next one have been waited for, the last one of the
-// tile after wait_group 0.
+// k-iterations [ki0, ki1) of one tile at NN token columns, walked as a flat sequence of k-blocks (two per stage, the
+// last stage of a tile may hold one).  Per k16 slice: convert the gate and up fragments of this warpgroup's rows from
+// registers, then issue their two MMAs (A registers, B = token tile of the stage).  Two slices are in flight: the
+// conversion of slice n runs while the MMAs of slice n - 1 execute (wait_group 1).  The next k-block's words are loaded
+// after the MMAs of the last slice are issued, into the registers of the current block's (now dead) words: no
+// shared-memory load sits between a wait and the next MMAs, and at 64 columns nothing spills.  A stage is released once
+// the MMAs of the next one have been waited for, the last one of the tile after wait_group 0.  Waiting for the next stage
+// only after slice 0 keeps the order safe with two stages: by then the previous stage has been released.
 template <class C, int NN>
 B200_DEVICE void w4_tile(const FusedArgs& a, FTables* tb, const uint8_t* smem, int KB, int ki0, int ki1,
                          float (&acc)[2][C::TN / 2], uint32_t& itc) {
   constexpr int WQ = C::WD;
-  constexpr bool SC = C::TN < 64;
-  const int lane = threadIdx.x & 31;
-  const int r0 = (((int)threadIdx.x >> 7) - C::MMA_WARP0 / 4) * 64 + (((int)threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
-  const int t = lane & 3;
+  const uint32_t u = threadIdx.x - C::MMA_WARP0 * 32;   // consumer thread, 0..255 (w4_layout.cuh)
   const bool lead = (threadIdx.x & 127) == 0;
   const uint32_t smem_u = smem_u32(smem);
   int pend = -1;   // stage whose last MMAs may still be in flight
@@ -362,40 +362,57 @@ B200_DEVICE void w4_tile(const FusedArgs& a, FTables* tb, const uint8_t* smem, i
   // register allocator has to give the two buffers distinct registers and ptxas need not serialise the wgmmas.
   uint32_t fa[2][2][4] = {};
   acc_fence(acc);
-  for (int ki = ki0; ki < ki1; ++ki, ++itc) {
-    const int s = itc % C::STAGES;
-    f_wait<true>(&tb->full[s], (itc / C::STAGES) & 1);
-    const int kb0 = ki * 2;
-    const int nkb = (KB - kb0) < 2 ? (KB - kb0) : 2;
-    const uint32_t raw = smem_u + s * C::STAGE;
-    const uint32_t sb = raw + C::A_STAGE;
-    for (int kk = 0; kk < nkb; ++kk) {
-      const uint32_t bbase = sb + kk * (uint32_t)((NN >> 3) * 1024);
-      W4Slice cur;
-      w4_load<WQ, SC>(cur, raw, a.w4_tile_bytes, kk, 0, r0);
+  uint32_t it = itc;
+  int ki = ki0, kk = 0, s = it % C::STAGES;
+  f_wait<true>(&tb->full[s], (it / C::STAGES) & 1);
+  W4Block cur;
+  w4_load<WQ>(cur, smem_u + s * C::STAGE, a.w4_tile_bytes, 0, u);
+  while (true) {
+    const int nkb = (KB - 2 * ki) < 2 ? (KB - 2 * ki) : 2;
+    const bool last_of_stage = kk + 1 == nkb;
+    const bool more = !last_of_stage || ki + 1 < ki1;
+    const uint32_t bbase = smem_u + s * C::STAGE + C::A_STAGE + kk * (uint32_t)((NN >> 3) * 1024);
+    W4Block nxt;
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        W4Slice nxt;
-        if (ks < 3) w4_load<WQ, SC>(nxt, raw, a.w4_tile_bytes, kk, ks + 1, r0);
-        uint32_t (&f)[2][4] = fa[ks & 1];
-        w4_convert<WQ, SC>(f, cur, raw, a.w4_tile_bytes, kk, ks, r0, t);
-        const uint64_t bd = wgmma_desc_sw128(bbase + ks * 32, 1024);
-        const uint32_t accum = (ki > ki0 || kk > 0 || ks > 0) ? 1u : 0u;
-        wgmma_fence();
-        WgmmaRS<NN, 0>::mma(acc[0], f[0], bd, accum);
-        WgmmaRS<NN, 0>::mma(acc[1], f[1], bd, accum);
-        wgmma_commit();
-        wgmma_wait<1>();
-        frag_hold(fa[(ks + 1) & 1]);   // the previous slice's MMAs are complete: its buffer may be overwritten now
-        if (pend >= 0) {
-          if (lead) mbar_arrive(&tb->empty[pend]);
-          pend = -1;
+    for (int ks = 0; ks < 4; ++ks) {
+      uint32_t (&f)[2][4] = fa[ks & 1];
+      w4_convert<WQ>(f, cur, ks);
+      const uint64_t bd = wgmma_desc_sw128(bbase + ks * 32, 1024);
+      const uint32_t accum = (ki > ki0 || kk > 0 || ks > 0) ? 1u : 0u;
+      wgmma_fence();
+      WgmmaRS<NN, 0>::mma(acc[0], f[0], bd, accum);
+      WgmmaRS<NN, 0>::mma(acc[1], f[1], bd, accum);
+      wgmma_commit();
+      if (ks == 3) {   // after the tile's last k-block this reloads the current one, unused: no branch around the load
+        uint32_t ns = s;
+        int nkk = more ? kk + 1 : kk;
+        if (last_of_stage && more) {
+          ns = (it + 1) % C::STAGES;
+          nkk = 0;
+          f_wait<true>(&tb->full[ns], ((it + 1) / C::STAGES) & 1);
         }
-        if (ks < 3) cur = nxt;
+        w4_load<WQ>(nxt, smem_u + ns * C::STAGE, a.w4_tile_bytes, nkk, u);
+      }
+      wgmma_wait<1>();
+      frag_hold(fa[(ks + 1) & 1]);   // the previous slice's MMAs are complete: its buffer may be overwritten now
+      if (pend >= 0) {
+        if (lead) mbar_arrive(&tb->empty[pend]);
+        pend = -1;
       }
     }
-    pend = s;
+    if (last_of_stage) {
+      pend = s;
+      ++it;
+      ++ki;
+      kk = 0;
+      s = it % C::STAGES;
+    } else {
+      ++kk;
+    }
+    if (!more) break;
+    cur = nxt;
   }
+  itc = it;
   wgmma_wait<0>();
   acc_fence(acc);
   if (lead && pend >= 0) mbar_arrive(&tb->empty[pend]);

@@ -103,8 +103,8 @@ struct b200moe_layer {
   uint8_t* w2t = nullptr;   // tiled: [E][J2][KB2][16 KB], or paired [E][J2/2][KB2][2][16 KB] when w2_paired
   int w2_paired = 0;
   // 4-bit weight formats (W4A16): wq 0 none, 1 int4 (uint4b8, fp16 group-32 scales), 2 nvfp4 (e4m3 group-16
-  // scales + f32 global), 3 mxfp4 (e8m0 group-32 scales).  Tiles are [128 rows x 64 cols]: 4096 B of nibbles
-  // ([2 col-groups][128 rows][16 B]) followed by w4_scale_bytes of scales; MMA operands are fp16.
+  // scales + f32 global), 3 mxfp4 (e8m0 group-32 scales).  Tiles are [128 rows x 64 cols]: 4096 B of nibbles followed
+  // by w4_scale_bytes of scales, both in the fused kernel's wgmma fragment order (w4_layout.cuh); MMA operands are fp16.
   int wq = 0;
   int w4_tile_bytes = 0, w4_scale_bytes = 0;
   int w13_interleaved = 0;   // activation_type 1 only: gate/up rows interleaved in the checkpoint (de-interleaved at ingest)

@@ -8,6 +8,7 @@
 //        of output features [128j,128j+128) is followed by the matching up tile.
 #include "common.cuh"
 #include "moe_internal.cuh"
+#include "w4_layout.cuh"
 
 namespace b200 {
 
@@ -105,44 +106,34 @@ __global__ void __launch_bounds__(256)
 
 // ---------------------------------------------------------------------------------- 4-bit formats
 // raw: packed nibbles u8 [E][N][K/2] (low nibble = even k; reference quant_utils.py:493-512 / nvfp4_utils.py:64-88)
-// tiled: [E][J][KB][2][tile]: tile = nibbles [2 col-groups of 32][128 rows][16 B] + scales.
-// INT4 words are nibble-permuted so that (nibble j, nibble j+4) of a 32-bit word are elements (2j, 2j+1): one
-// shift + one LOP3 then yields an fp16x2 pair (Marlin-style magic-number dequantisation).
+// tiled: [E][J][KB][2][tile]: tile = 4096 B of nibbles in the consumers' wgmma fragment order + scales (w4_layout.cuh).
+// One thread per nibble word: it gathers the word's 8 codes, two columns per source byte.
 __global__ void __launch_bounds__(256)
     tile_w4_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int E, int J, int KB, int rows_per_expert,
-                   int up_row_off, int tile_rows, int64_t row_bytes, int tile_bytes, int permute, int row_step) {
-  const int64_t n_units = (int64_t)E * J * KB * 2 * 256;  // 256 16-byte units per tile
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_units; i += (int64_t)gridDim.x * blockDim.x) {
+                   int up_row_off, int tile_rows, int64_t row_bytes, int tile_bytes, int e2m1, int row_step) {
+  const int64_t n_words = (int64_t)E * J * KB * 2 * (W4_NIBBLE_BYTES / 4);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_words; i += (int64_t)gridDim.x * blockDim.x) {
     int64_t t = i;
-    const int r = t % 128;  t /= 128;
-    const int g = t % 2;  t /= 2;
+    const int wd = t % (W4_NIBBLE_BYTES / 4);  t /= W4_NIBBLE_BYTES / 4;
     const int na = t % 2;  t /= 2;
     const int kb = t % KB;  t /= KB;
     const int j = t % J;  t /= J;
     const int e = (int)t;
-    const int64_t srow = (int64_t)e * rows_per_expert + (na ? up_row_off : 0) + ((int64_t)j * tile_rows + r) * row_step;
-    uint4 v = *reinterpret_cast<const uint4*>(src + srow * row_bytes + (int64_t)kb * 32 + g * 16);
-    if (permute) {
-      uint32_t* w = reinterpret_cast<uint32_t*>(&v);
+    uint32_t v = 0;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const uint32_t x = w[q];
-        uint32_t y = 0;
-#pragma unroll
-        for (int p = 0; p < 4; ++p) {
-          y |= ((x >> (8 * p)) & 0xFu) << (4 * p);             // element 2p   -> nibble p
-          y |= ((x >> (8 * p + 4)) & 0xFu) << (4 * (p + 4));   // element 2p+1 -> nibble p+4
-        }
-        w[q] = y;
-      }
+    for (int reg = 0; reg < 4; ++reg) {
+      const int r = w4_row(wd, reg), c = w4_col(wd, reg, 0);   // columns c (low nibble) and c + 1 (high nibble)
+      const int64_t srow = (int64_t)e * rows_per_expert + (na ? up_row_off : 0) + ((int64_t)j * tile_rows + r) * row_step;
+      const uint32_t by = src[srow * row_bytes + (int64_t)kb * 32 + c / 2];
+      v |= w4_code_bits(e2m1, reg, 0, by & 0xFu) | w4_code_bits(e2m1, reg, 1, by >> 4);
     }
     const int64_t tile = (((int64_t)(e * J + j) * KB + kb) * 2 + na);
-    *reinterpret_cast<uint4*>(dst + tile * tile_bytes + (g * 128 + r) * 16) = v;
+    reinterpret_cast<uint32_t*>(dst + tile * tile_bytes)[wd] = v;
   }
 }
 
-// scales of one tile: fmt 1: fp16 [2 groups(32)][128] from act-dtype scales [E][N][K/gs]; fmt 2: e4m3 [4 groups(16)][128]
-// from [E][N][K/16]; fmt 3: e8m0 [2][128] from [E][N][K/32]
+// scales of one tile (w4_layout.cuh): fmt 1: fp16, 2 groups of 32 columns, from act-dtype scales [E][N][K/gs]; fmt 2:
+// e4m3, 4 groups of 16, from [E][N][K/16]; fmt 3: e8m0, 2 groups of 32, from [E][N][K/32]
 __global__ void __launch_bounds__(256)
     tile_w4_scales_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int E, int J, int KB,
                           int rows_per_expert, int up_row_off, int tile_rows, int K, int fmt, int gs, int src_fp16,
@@ -159,7 +150,7 @@ __global__ void __launch_bounds__(256)
     const int r = u % 128, g = u / 128;
     const int64_t srow = (int64_t)e * rows_per_expert + (na ? up_row_off : 0) + ((int64_t)j * tile_rows + r) * row_step;
     const int64_t tile = (((int64_t)(e * J + j) * KB + kb) * 2 + na);
-    uint8_t* d = dst + tile * tile_bytes + 4096;
+    uint8_t* d = dst + tile * tile_bytes + W4_NIBBLE_BYTES + w4_scale_off(fmt, r, g);
     if (fmt == 1) {
       const int col = kb * 64 + g * 32;
       const int64_t si = srow * (K / gs) + col / gs;
@@ -168,11 +159,11 @@ __global__ void __launch_bounds__(256)
         f = __half2float(reinterpret_cast<const __half*>(src)[si]);
       else
         f = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(src)[si]);
-      reinterpret_cast<__half*>(d)[g * 128 + r] = __float2half_rn(f);
+      *reinterpret_cast<__half*>(d) = __float2half_rn(f);
     } else if (fmt == 2) {
-      d[g * 128 + r] = src[srow * (K / 16) + kb * 4 + g];
+      *d = src[srow * (K / 16) + kb * 4 + g];
     } else {
-      d[g * 128 + r] = src[srow * (K / 32) + kb * 2 + g];
+      *d = src[srow * (K / 32) + kb * 2 + g];
     }
   }
 }
@@ -200,12 +191,12 @@ int repack_weights_w4(b200moe_layer* L, int e0, int ne, const void* w13, const v
   }
   uint8_t* d13 = L->w13t + e0 * pe13;
   uint8_t* d2 = L->w2t + e0 * pe2;
-  const int perm = (L->wq == 1);
+  const int e2m1 = (L->wq != 1);
   const int il = L->w13_interleaved;   // gate = even rows, up = odd rows of w13 (de-interleaved here)
   tile_w4_kernel<<<2048, 256, 0, st>>>(reinterpret_cast<const uint8_t*>(w13), d13, ne, L->J1, KB1, L->N1,
-                                      il ? 1 : L->I, 128, (int64_t)L->H / 2, tb, perm, il ? 2 : 1);
+                                      il ? 1 : L->I, 128, (int64_t)L->H / 2, tb, e2m1, il ? 2 : 1);
   tile_w4_kernel<<<2048, 256, 0, st>>>(reinterpret_cast<const uint8_t*>(w2), d2, ne, L->J2 / 2, KB2, L->H, 128, 256,
-                                      (int64_t)L->I / 2, tb, perm, 1);
+                                      (int64_t)L->I / 2, tb, e2m1, 1);
   const int gs = L->cfg.groupK > 0 ? L->cfg.groupK : 32;
   tile_w4_scales_kernel<<<1024, 256, 0, st>>>(reinterpret_cast<const uint8_t*>(s13), d13, ne, L->J1, KB1, L->N1,
                                              il ? 1 : L->I, 128, L->H, L->wq, gs, L->act_dtype == B200_ACT_FP16, tb,
@@ -303,7 +294,8 @@ B200_DEVICE void store_fp16x32(uint8_t* dst_tile, int r, int chunk0, const float
   }
 }
 
-// dequant-layout tiles ([128 x 64]: 4 KB nibbles [2 col groups][128 rows][16 B] + scales) -> fp16 tiles, same tile order
+// 4-bit tiles (w4_layout.cuh) -> fp16 tiles, same tile order.  Thread (g, r) expands columns [32g, 32g + 32) of row r:
+// the 8 nibble words of slices 2g and 2g + 1 that hold row r, four codes from each.
 __global__ void __launch_bounds__(256)
     dequant_w4_tiles_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int64_t n_tiles, int tiles_per_expert,
                             int tile_bytes, int wq, const float* __restrict__ gscale, int gs_per_expert) {
@@ -311,40 +303,32 @@ __global__ void __launch_bounds__(256)
     const int64_t t = i >> 8;
     const int u = (int)(i & 255), g = u >> 7, r = u & 127;
     const uint8_t* tile = src + t * tile_bytes;
-    const uint8_t* sc = tile + 4096;
-    const uint4 q = *reinterpret_cast<const uint4*>(tile + (g * 128 + r) * 16);
-    const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-    float v[32];
+    const uint8_t* sc = tile + W4_NIBBLE_BYTES;
+    float s2[2];   // scales of columns [32g, 32g + 16) and [32g + 16, 32g + 32)
     if (wq == 1) {
-      const float s = __half2float(reinterpret_cast<const __half*>(sc)[g * 128 + r]);
-#pragma unroll
-      for (int wi = 0; wi < 4; ++wi)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {   // permuted words: nibbles (j, j + 4) = elements (2j, 2j + 1)
-          v[wi * 8 + 2 * j] = (float)((int)((w[wi] >> (4 * j)) & 0xFu) - 8) * s;
-          v[wi * 8 + 2 * j + 1] = (float)((int)((w[wi] >> (4 * j + 16)) & 0xFu) - 8) * s;
-        }
+      s2[0] = s2[1] = __half2float(*reinterpret_cast<const __half*>(sc + w4_scale_off(1, r, g)));
+    } else if (wq == 2) {
+      const int na = (int)(t & 1);
+      const int e = (int)(t / tiles_per_expert);
+      const float gsc = gscale[(size_t)e * gs_per_expert + (gs_per_expert == 2 ? na : 0)];
+      const __half_raw h0 = __nv_cvt_fp8_to_halfraw(sc[w4_scale_off(2, r, 2 * g)], __NV_E4M3);
+      const __half_raw h1 = __nv_cvt_fp8_to_halfraw(sc[w4_scale_off(2, r, 2 * g + 1)], __NV_E4M3);
+      s2[0] = __half2float(*reinterpret_cast<const __half*>(&h0)) * gsc;
+      s2[1] = __half2float(*reinterpret_cast<const __half*>(&h1)) * gsc;
     } else {
-      float s2[2];
-      if (wq == 2) {
-        const int na = (int)(t & 1);
-        const int e = (int)(t / tiles_per_expert);
-        const float gsc = gscale[(size_t)e * gs_per_expert + (gs_per_expert == 2 ? na : 0)];
-        const __half_raw h0 = __nv_cvt_fp8_to_halfraw(sc[(2 * g) * 128 + r], __NV_E4M3);
-        const __half_raw h1 = __nv_cvt_fp8_to_halfraw(sc[(2 * g + 1) * 128 + r], __NV_E4M3);
-        s2[0] = __half2float(*reinterpret_cast<const __half*>(&h0)) * gsc;
-        s2[1] = __half2float(*reinterpret_cast<const __half*>(&h1)) * gsc;
-      } else {
-        s2[0] = s2[1] = __uint_as_float((uint32_t)sc[g * 128 + r] << 23);   // e8m0 -> 2^(E-127)
+      s2[0] = s2[1] = __uint_as_float((uint32_t)sc[w4_scale_off(3, r, g)] << 23);   // e8m0 -> 2^(E-127)
+    }
+    float v[32];
+#pragma unroll
+    for (int c0 = 0; c0 < 32; c0 += 2) {
+      const int c = 32 * g + c0;
+      const uint32_t w = reinterpret_cast<const uint32_t*>(tile)[w4_word(r, c)];
+      const int reg = w4_reg(r, c);
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const uint32_t q = w4_code(wq != 1, reg, e, w);
+        v[c0 + e] = (wq == 1 ? (float)((int)q - 8) : c_e2m1[q]) * s2[c0 >> 4];
       }
-#pragma unroll
-      for (int wi = 0; wi < 4; ++wi)
-#pragma unroll
-        for (int b = 0; b < 4; ++b) {
-          const uint32_t byte = (w[wi] >> (8 * b)) & 0xFFu;
-          v[wi * 8 + 2 * b] = c_e2m1[byte & 15u] * s2[wi >> 1];
-          v[wi * 8 + 2 * b + 1] = c_e2m1[byte >> 4] * s2[wi >> 1];
-        }
     }
     store_fp16x32(dst + t * TILE_BYTES, r, g * 4, v);
   }
