@@ -227,6 +227,39 @@ int b200_mla_decode_sparse(void* stream, const void* q_nope, const void* q_pe, c
                            const int32_t* topk_indices, int topk, const int32_t* req_id, const int32_t* page_table,
                            int max_pages, int num_tokens, int num_heads, int page_size, float sm_scale, int num_splits,
                            void* workspace, void* out, float* lse, const void* w_uv, void* out_v);
+/* DeepSeek-V4 sparse attention decode (the reference's FlashMLA call with indices / extra_k_cache / attn_sink,
+ * models/deepseek_v4/nvidia/flashmla.py:151-244).  Head dim 512 = 448 NoPE + 64 RoPE dims; one cache row is both K and V.
+ * q bf16 [num_tokens, num_heads, 512].  Both caches hold 584-byte tokens per block (flashmla_sparse.py:76-85): block b starts at
+ * b * block_stride bytes, token p's data (448 e4m3 | 64 bf16 rope) at + p * 576, its scale record (7 ue8m0 bytes, one per 64
+ * NoPE dims, then a pad byte) at + block_size * 576 + p * 8; a NoPE value is bf16(e4m3) * 2^(s - 127).  Keys of token t:
+ * swa_indices[t, :swa_lens[t]] (int32 [num_tokens, swa_topk], global slots of swa_cache) followed, when extra_cache is given,
+ * by extra_indices[t, :extra_lens[t]] (global slots of extra_cache, its own block size); lengths are clamped to [0, topk].
+ * A slot resolves to (slot / block_size, slot % block_size); a slot < 0 or >= num_blocks * block_size is no key.
+ * s_j = sm_scale * q . k_j; out bf16 [num_tokens, num_heads, 512] = sum_j p_j k_j with the softmax over the valid keys, and
+ * with attn_sink (f32 [num_heads], or NULL) m' = max(m, sink_h), l' = l e^(m - m') + e^(sink_h - m'), out = acc e^(m - m') / l',
+ * folded in once after the split merge.  A token with no valid key gets out = 0.  Workspace:
+ * b200_mla_decode_workspace_bytes(num_tokens, num_heads, num_splits).  No allocation, no synchronisation (graph-capturable).
+ * B200_ERR_INVALID, nothing launched: a NULL required pointer, q / caches / workspace / out not 16-byte aligned, index and
+ * length arrays not 4-byte aligned, num_tokens outside [1, 65535], num_heads outside [1, 128], topk < 1, a block stride below
+ * block_size * 584 or not a multiple of 16, num_splits outside [1, 512]. */
+int b200_dsv4_sparse_decode(void* stream, const void* q, int num_tokens, int num_heads, const void* swa_cache,
+                            int swa_block_size, int swa_num_blocks, int64_t swa_block_stride, const int32_t* swa_indices,
+                            int swa_topk, const int32_t* swa_lens, const void* extra_cache, int extra_block_size,
+                            int extra_num_blocks, int64_t extra_block_stride, const int32_t* extra_indices, int extra_topk,
+                            const int32_t* extra_lens, const float* attn_sink, float sm_scale, int num_splits,
+                            void* workspace, void* out);
+/* DeepSeek-V4 q-norm + RoPE + cache insert, one launch (the reference's fused_deepseek_v4_qnorm_rope_kv_rope_quant_insert,
+ * csrc/libtorch_stable/fused_deepseek_v4_qnorm_rope_kv_insert_kernel.cu).  q bf16 [num_tokens, num_heads, 512]: per-head RMSNorm
+ * without weight (eps), then GPT-J pair RoPE of dims 448-511, all in fp32, rounded once into q_out bf16
+ * [num_tokens, q_head_padded, 512]; heads num_heads .. q_head_padded - 1 are written as zeros.  kv bf16 [num_tokens, 512]
+ * (after kv_norm): RoPE of dims 448-511; NoPE dims quantised per 64 with scale 2^ceil(log2(max(amax, 1e-4) / 448)) to e4m3 and
+ * a ue8m0 byte, written with the bf16 rope dims to row slot_mapping[t] (int64; < 0 or past the cache: nothing written) of the
+ * 584-byte cache laid out as in b200_dsv4_sparse_decode.  positions int64 [num_tokens] (clamped to [0, max_position));
+ * cos_sin_cache f32 [max_position, 64] = cos | sin. */
+int b200_dsv4_qnorm_rope_kv_insert(void* stream, const void* q, const void* kv, const int64_t* positions,
+                                   const float* cos_sin_cache, int max_position, const int64_t* slot_mapping, void* cache,
+                                   int block_size, int num_blocks, int64_t block_stride, void* q_out, int num_tokens,
+                                   int num_heads, int q_head_padded, float eps);
 /* The MLA decode kernel's neighbours (SURVEY.md 8f row 3), bf16:
  *  b200_mla_rope_cache_write  RoPE of q_pe [T,Hq,64] and k_pe [T,64] in place (rotary_embedding/base.py:161-201; cos_sin_cache
  *      bf16 [max_pos,64] = cos | sin; is_neox 0 = GPT-J pairs (DeepSeek), 1 = NeoX halves) fused with concat_and_cache_mla

@@ -165,9 +165,14 @@ __global__ void __launch_bounds__(128) decode_merge_kernel(const float* __restri
 
 // merge for many splits (tensor-core MLA): one CTA per (b, head), thread = float4 of the 512 dims; the split
 // weights are computed once in shared memory, partial rows are read 8 splits at a time (independent loads)
+// SINK (DeepSeek-V4 attn_sink, f32 [Hq], natural-log units, row w is head w % Hq): folded in once, after every split is
+// merged: m' = max(m, sink), l' = l e^(m - m') + e^(sink - m'), out = acc e^(m - m') / l'.  A row with no valid key keeps
+// l = 0 and gets out = 0; sink = -inf gives the bits of the merge without a sink.
+template <bool SINK>
 __global__ void __launch_bounds__(128) mla_merge_kernel(const float* __restrict__ part_o,
                                                        const float* __restrict__ part_ml, int num_splits,
-                                                       __nv_bfloat16* __restrict__ out, float* __restrict__ lse) {
+                                                       __nv_bfloat16* __restrict__ out, float* __restrict__ lse,
+                                                       const float* __restrict__ sink, int Hq) {
   __shared__ float wgt[512];
   __shared__ float red[4];
   const int w = blockIdx.x, tid = threadIdx.x;
@@ -209,7 +214,12 @@ __global__ void __launch_bounds__(128) mla_merge_kernel(const float* __restrict_
       acc.w = fmaf(f[u], v[u].w, acc.w);
     }
   }
-  const float inv = lsum > 0.f ? 1.f / lsum : 0.f;
+  float inv = lsum > 0.f ? 1.f / lsum : 0.f;
+  if (SINK && lsum > 0.f) {   // exp2 domain: the partials' m are in log2 units
+    const float sk = sink[w % Hq] * 1.4426950408889634f, m2 = fmaxf(mx, sk);
+    const float f = exp2f(mx - m2);
+    inv = f / fmaf(lsum, f, exp2f(sk - m2));
+  }
   __nv_bfloat162 a = __floats2bfloat162_rn(acc.x * inv, acc.y * inv), c = __floats2bfloat162_rn(acc.z * inv, acc.w * inv);
   uint2 pk;
   pk.x = *reinterpret_cast<uint32_t*>(&a);
@@ -225,7 +235,8 @@ static int mla_merge(cudaStream_t st, const float* po, const float* pml, int row
   if (w_uv)
     launch_mla_merge_vup(st, po, pml, rows, num_splits, num_heads, w_uv, out_v, out, lse);
   else if (num_splits <= 512)
-    mla_merge_kernel<<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse);
+    mla_merge_kernel<false><<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse,
+                                                             nullptr, num_heads);
   else
     decode_merge_kernel<512><<<(rows * num_heads + 3) / 4, 128, 0, st>>>(po, pml, rows * num_heads, num_splits,
                                                                         reinterpret_cast<__nv_bfloat16*>(out), lse);
@@ -308,6 +319,50 @@ int b200_mla_decode_sparse(void* stream, const void* q_nope, const void* q_pe, c
                                       max_pages, num_tokens, num_heads, page_size, sm_scale, num_splits, po, pml);
   if (rc) return rc;
   return mla_merge(st, po, pml, num_tokens, num_heads, num_splits, out, lse, w_uv, out_v);
+}
+
+int b200_dsv4_sparse_decode(void* stream, const void* q, int num_tokens, int num_heads, const void* swa_cache,
+                            int swa_block_size, int swa_num_blocks, int64_t swa_block_stride, const int32_t* swa_indices,
+                            int swa_topk, const int32_t* swa_lens, const void* extra_cache, int extra_block_size,
+                            int extra_num_blocks, int64_t extra_block_stride, const int32_t* extra_indices, int extra_topk,
+                            const int32_t* extra_lens, const float* attn_sink, float sm_scale, int num_splits,
+                            void* workspace, void* out) {
+  auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+  auto a4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; };
+  // a cache: 16-byte aligned, blocks of block_size x 584 bytes at a 16-byte multiple stride
+  auto cache_ok = [&](const void* c, int bs, int nb, int64_t stride) {
+    return c && a16(c) && bs > 0 && nb > 0 && stride >= (int64_t)bs * 584 && stride % 16 == 0;
+  };
+  const bool extra = extra_cache != nullptr;
+  if (!q || !a16(q) || num_tokens <= 0 || num_tokens > 65535 || num_heads <= 0 || num_heads > 128 ||
+      !cache_ok(swa_cache, swa_block_size, swa_num_blocks, swa_block_stride) || !swa_indices || !a4(swa_indices) ||
+      swa_topk < 1 || !swa_lens || !a4(swa_lens) ||
+      (extra && (!cache_ok(extra_cache, extra_block_size, extra_num_blocks, extra_block_stride) || !extra_indices ||
+                 !a4(extra_indices) || extra_topk < 1 || !extra_lens || !a4(extra_lens))) ||
+      (attn_sink && !a4(attn_sink)) || num_splits <= 0 || num_splits > 512 || !workspace || !a16(workspace) || !out ||
+      !a16(out)) {
+    set_error("b200_dsv4_sparse_decode: bad argument (num_tokens <= 65535, num_heads <= 128, topk >= 1, 16-byte aligned q, "
+              "caches, workspace and out, block stride >= block_size * 584 and a multiple of 16, 1 <= num_splits <= 512; "
+              "extra_cache given: its indices, lengths and shape too)");
+    return B200_ERR_INVALID;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* po = reinterpret_cast<float*>(workspace);
+  float* pml = po + (size_t)num_tokens * num_heads * num_splits * 512;
+  int rc = launch_dsv4_sparse_tc(st, q, swa_cache, swa_block_size, swa_num_blocks, swa_block_stride, swa_indices, swa_topk,
+                                 swa_lens, extra_cache, extra_block_size, extra_num_blocks, extra_block_stride,
+                                 extra ? extra_indices : nullptr, extra_topk, extra_lens, num_tokens, num_heads, sm_scale,
+                                 num_splits, po, pml);
+  if (rc) return rc;
+  auto bo = reinterpret_cast<__nv_bfloat16*>(out);
+  if (attn_sink)
+    mla_merge_kernel<true><<<num_tokens * num_heads, 128, 0, st>>>(po, pml, num_splits, bo, nullptr, attn_sink, num_heads);
+  else
+    mla_merge_kernel<false><<<num_tokens * num_heads, 128, 0, st>>>(po, pml, num_splits, bo, nullptr, nullptr, num_heads);
+  ++g_launches;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "dsv4 merge launch");
+  return 0;
 }
 
 int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void* v_cache, const int32_t* seq_lens,

@@ -32,6 +32,18 @@
 // fp8_ds_mla (656 bytes per token: 512 e4m3, four fp32 scales, one per 128 dims, 64 bf16 rope dims; reference
 // v1/attention/backends/mla/flashmla_sparse.py:63-72), widened to bf16 by the loaders.
 //
+// DeepSeek-V4 sparse decode (V4): head dim 512 = 448 NoPE + 64 RoPE dims, and the key row is also the value row (shared-KV
+// MQA, no absorb).  The keys of token t are the concatenation main || extra: swa_indices[t, :swa_lens[t]] (global slots of the
+// sliding-window cache) followed by extra_indices[t, :extra_lens[t]] (global slots of the compressed cache, its own block
+// size); a slot resolves to (block = slot / block_size, pos = slot % block_size), and a slot < 0 or >= num_blocks * block_size
+// is no key (zero-filled, masked as above).  Both caches hold 584-byte tokens laid out per block (reference
+// flashmla_sparse.py:76-85, _read_fp8_ds_mla_cache in tests/kernels/attention/test_rocm_triton_attn_dsv4.py:125-147): the
+// block's block_size x 576 data bytes (448 e4m3 | 64 bf16 rope) come first, then block_size x 8 scale bytes (7 ue8m0, one per
+// 64 NoPE dims, and a pad byte); blocks are block_stride bytes apart.  QK^T runs over 8 k-blocks (kb 7 = rope, by cp.async),
+// the loaders widen kb 0-6 to bf16(e4m3) * 2^(s - 127) (exact), and value quarter p is k-blocks 2p, 2p + 1 (quarter 3 = NoPE
+// 384-447 | rope).  The q row is the 512-dim [T, Hq, 512] row, read through q_nope.  The attention sink is folded in by the
+// split merge (attention.cu).
+//
 // Warp roles (384 threads): warps 0-3 / 4-7 consumer warpgroups (MMA + softmax + epilogue), warps 8-11 loaders
 // (16-byte gathers of q rows / paged KV rows -> swizzled smem, generic->async proxy fence).
 // The op contract is reference csrc/libtorch_stable/attention/mla/sm100_cutlass_mla_kernel.cu:225-262.
@@ -64,6 +76,16 @@ struct MlaBars {
   uint32_t kvalid[2][4];
 };
 
+// V4: the parts of the key lists the kernel's shared arguments do not carry (the main list's cache, index rows, lengths,
+// block size and block count go in kv, topk_idx, seq_lens, page_size and max_pages); extra_idx == nullptr: no extra list
+struct Dsv4Keys {
+  const void* extra_kv;
+  const int32_t* extra_idx;
+  const int32_t* extra_lens;
+  int extra_topk, extra_block, extra_blocks;
+  int64_t main_stride, extra_stride;   // block strides in bytes
+};
+
 B200_DEVICE void mla_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -86,6 +108,12 @@ B200_DEVICE uint4 fp8x8_to_bf16x8(uint2 v) {
     }
   }
   return make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+// V4: scale of NoPE k-block kb of a 584-byte row, 2^(s - 127) for its ue8m0 byte s (s = 0 is the fp32 subnormal 2^-127)
+B200_DEVICE float ue8m0_scale(uint2 rec, int kb) {
+  const uint32_t s = ((kb < 4 ? rec.x : rec.y) >> (8 * (kb & 3))) & 0xFFu;
+  return __uint_as_float(s ? s << 23 : 0x00400000u);
 }
 
 // eight e4m3 bytes of an fp8_ds_mla row -> eight bf16 bf16(float(e4m3) * scale): the fp32 product, rounded once to bf16
@@ -113,14 +141,17 @@ B200_DEVICE uint4 fp8x8_scaled_to_bf16x8(uint2 v, float scale) {
 // rows = heads, one limit for every row), which keeps the single-token decode free of the per-row bookkeeping.
 // SPARSE: blockIdx.z is a query token, its keys come from topk_idx (see the header); with KV8 the cache is fp8_ds_mla (the
 // queries are bf16 then, q8 = 0).  The three trailing arguments are read by the sparse instantiations only.
-template <bool KV8, bool SPEC, bool SPARSE>
+// V4 (with KV8 && SPARSE): the DeepSeek-V4 cache (see the header).  kv / topk_idx / topk / seq_lens / page_size / max_pages are
+// the main list's cache, index rows, row width, lengths, block size and block count; v4 holds the rest.
+template <bool KV8, bool SPEC, bool SPARSE, bool V4>
 __global__ void __launch_bounds__(MLA_THREADS, 1)
     mla_decode_tc_kernel(const void* __restrict__ q_nope_v, const void* __restrict__ q_pe_v,
                          const void* __restrict__ kv_v, const int32_t* __restrict__ seq_lens,
                          const int32_t* __restrict__ page_table, int Hq, int page_size, int max_pages,
                          float scale_log2, int num_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
                          int q8, float out_scale, int tiles_per_cta, int Q_, int Qg_,
-                         const int32_t* __restrict__ topk_idx, const int32_t* __restrict__ req_id, int topk) {
+                         const int32_t* __restrict__ topk_idx, const int32_t* __restrict__ req_id, int topk,
+                         Dsv4Keys v4) {
   const __nv_bfloat16* q_nope = reinterpret_cast<const __nv_bfloat16*>(q_nope_v);
   const __nv_bfloat16* q_pe = reinterpret_cast<const __nv_bfloat16*>(q_pe_v);
   const __nv_bfloat16* kv = reinterpret_cast<const __nv_bfloat16*>(kv_v);
@@ -138,8 +169,10 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
   const int nrows = qn * Hq;                         // MMA rows that carry a query
   const size_t row0 = (size_t)(b * Q + qg * Qg) * Hq;   // q / output row of MMA row 0
   // keys of the group's last draft token: the most any row of this CTA sees (all of them when Q = 1)
-  // (SPARSE: the entries of the token's index row)
-  const int S = SPARSE ? topk : SPEC ? seq_lens[b] - Q + qg * Qg + qn : seq_lens[b];
+  // (SPARSE: the entries of the token's index row; V4: the main entries then the extra ones)
+  const int n_main = V4 ? min(max(seq_lens[b], 0), topk) : 0;
+  const int S = V4 ? n_main + (v4.extra_idx ? min(max(v4.extra_lens[b], 0), v4.extra_topk) : 0)
+                   : SPARSE ? topk : SPEC ? seq_lens[b] - Q + qg * Qg + qn : seq_lens[b];
   const int t_first = split * tiles_per_cta * MLA_TOK;
   // this CTA walks n_tiles consecutive 128-token tiles of the request with an online softmax: O stays in registers,
   // partial (O, m, l) leave the CTA once
@@ -155,8 +188,10 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
     return;
   }
 
+  // V4: no q_pe k-block; kb 7 is the rope block
+  constexpr int KB = V4 ? MLA_KB - 1 : MLA_KB, ROPE_KB = KB - 1;
   if (tid == 0) {
-    for (int i = 0; i < MLA_KB; ++i) mbar_init(&bars->full[i], 128);
+    for (int i = 0; i < KB; ++i) mbar_init(&bars->full[i], 128);
     for (int i = 0; i < MLA_QSTAGES; ++i) mbar_init(&bars->empty[i], 2);   // one arrival per consumer warpgroup
     mbar_init(&bars->s_full, 2);
     mbar_init(&bars->o_full, 2);
@@ -166,10 +201,10 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
   // row r is draft token j = r / Hq of the group (rows past its last token take that token's limit)
   if (SPEC && tid < 128) bars->row_off[tid] = (int8_t)(qn - 1 - min(tid / Hq, qn - 1));
   __syncthreads();
-  // k-block order of a tile: the seven blocks the PV MMA of THIS CTA does not read (the other CTAs' value dims and the
-  // rope block) come first — they can be refilled as soon as QK^T of the previous tile has completed, the two value
+  // k-block order of a tile: the seven (V4: six) blocks the PV MMA of THIS CTA does not read (the other CTAs' value dims and
+  // the rope block) come first — they can be refilled as soon as QK^T of the previous tile has completed, the two value
   // blocks only after its PV
-  constexpr int MLA_NV = MLA_DV / 64, MLA_NO = MLA_KB - MLA_NV;
+  constexpr int MLA_NV = MLA_DV / 64, MLA_NO = KB - MLA_NV;
   auto kb_of = [&](int j) { return j < MLA_NO ? (j < part * MLA_NV ? j : j + MLA_NV) : part * MLA_NV + (j - MLA_NO); };
 
   if (warp >= 8) {
@@ -187,8 +222,26 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
       const __nv_bfloat16* krow[8];
       const uint8_t* krow8[8];
       float kscale[8][4];   // SPARSE && KV8: the row's four fp8_ds_mla scales
+      uint2 kue[8];         // V4: the row's scale record, 7 ue8m0 bytes and a pad byte
       uint32_t vword = 0;   // SPARSE: this warp's word of the tile's valid mask
-      if (SPARSE) {
+      if (V4) {
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const int e = t0 + r0 + 16 * u;   // entry of the concatenated list main || extra
+          const bool extra = e >= n_main;
+          const int slot = e >= S ? -1 : !extra ? topk_idx[(size_t)b * topk + e]
+                                                : v4.extra_idx[(size_t)b * v4.extra_topk + (e - n_main)];
+          const int bs = extra ? v4.extra_block : page_size;
+          const bool ok = slot >= 0 && (int64_t)slot < (int64_t)(extra ? v4.extra_blocks : max_pages) * bs;
+          const uint8_t* blk = reinterpret_cast<const uint8_t*>(extra ? v4.extra_kv : kv_v) +
+                               (size_t)(ok ? slot / bs : 0) * (size_t)(extra ? v4.extra_stride : v4.main_stride);
+          const int pos = ok ? slot % bs : 0;
+          krow8[u] = ok ? blk + (size_t)pos * 576 : nullptr;
+          kue[u] = ok ? __ldg(reinterpret_cast<const uint2*>(blk + (size_t)bs * 576 + (size_t)pos * 8)) : make_uint2(0u, 0u);
+          const uint32_t bal = __ballot_sync(0xffffffffu, ok);
+          vword |= ((bal & 1u) | ((bal >> 7) & 2u) | ((bal >> 14) & 4u) | ((bal >> 21) & 8u)) << (4 * u);
+        }
+      } else if (SPARSE) {
         const int32_t* pt_row = page_table + (size_t)req_id[b] * max_pages;
 #pragma unroll
         for (int u = 0; u < 8; ++u) {
@@ -234,8 +287,8 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
             const int r = r0 + 16 * u;
-            // fp8_ds_mla: the rope block (kb 8) is bf16 and goes in by cp.async
-            kreg[buf][u] = krow8[u] && !(SPARSE && kb == 8)
+            // fp8_ds_mla: the rope block (kb 8, V4: kb 7) is bf16 and goes in by cp.async
+            kreg[buf][u] = krow8[u] && !(SPARSE && kb == ROPE_KB)
                                ? __ldg(reinterpret_cast<const uint2*>(krow8[u] + kb * 64 + c * 8)) : make_uint2(0u, 0u);
             qreg[buf][u] = make_uint2(0u, 0u);
             if (!SPARSE && q8 && r < nrows)
@@ -246,10 +299,10 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
 #pragma unroll
         for (int j = 0; j < MLA_PF - 1; ++j) issue(j, j);
 #pragma unroll
-        for (int j = 0; j < MLA_KB; ++j, ++qit) {
+        for (int j = 0; j < KB; ++j, ++qit) {
           const int kb = kb_of(j);
           const int s = qit % MLA_QSTAGES, buf = j % MLA_PF;
-          if (j + MLA_PF - 1 < MLA_KB) issue(j + MLA_PF - 1, (j + MLA_PF - 1) % MLA_PF);
+          if (j + MLA_PF - 1 < KB) issue(j + MLA_PF - 1, (j + MLA_PF - 1) % MLA_PF);
           if (ti > 0) mla_wait(j < MLA_NO ? &bars->s_full : &bars->o_full, (ti - 1) & 1);   // the block's previous readers are done
           if (SPARSE && j == 0 && lane == 0) {   // publish the mask once tile ti - 1's QK^T is done (see v_full)
             bars->kvalid[ti & 1][warp - 8] = vword;
@@ -270,12 +323,12 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
             }
             if (!SPARSE)
               *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(kreg[buf][u]);
-            else if (kb < 8)
+            else if (kb < ROPE_KB)
               *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) =
-                  fp8x8_scaled_to_bf16x8(kreg[buf][u], kscale[u][kb >> 1]);
+                  fp8x8_scaled_to_bf16x8(kreg[buf][u], V4 ? ue8m0_scale(kue[u], kb) : kscale[u][kb >> 1]);
             else
               cp_async16(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16),
-                         krow8[u] ? krow8[u] + 528 + c * 16 : kv_v, krow8[u] != nullptr);
+                         krow8[u] ? krow8[u] + (V4 ? 448 : 528) + c * 16 : kv_v, krow8[u] != nullptr);
           }
           if (SPARSE || !q8) asm volatile("cp.async.wait_all;" ::: "memory");
           fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
@@ -283,7 +336,7 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
         }
       } else {
         // cp.async (LDGSTS) straight into the swizzled tiles: no register staging; completion is signalled per k-block
-        for (int j = 0; j < MLA_KB; ++j, ++qit) {
+        for (int j = 0; j < KB; ++j, ++qit) {
           const int kb = kb_of(j);
           const int s = qit % MLA_QSTAGES;
           if (ti > 0) mla_wait(j < MLA_NO ? &bars->s_full : &bars->o_full, (ti - 1) & 1);
@@ -335,8 +388,8 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
       const int nt = min(MLA_TOK, S - (t_first + ti * MLA_TOK));
       // valid tokens of the tile per row (row h0 + 8r), t < ntr[r]
       const int ntr[2] = {S - (t_first + ti * MLA_TOK) - bars->row_off[h0], S - (t_first + ti * MLA_TOK) - bars->row_off[h0 + 8]};
-      // S = Q K^T over the nine k-blocks, in the order the loaders fill them
-      for (int j = 0; j < MLA_KB; ++j, ++qit) {
+      // S = Q K^T over the nine (V4: eight) k-blocks, in the order the loaders fill them
+      for (int j = 0; j < KB; ++j, ++qit) {
         const int kb = kb_of(j);
         const int s = qit % MLA_QSTAGES;
         mla_wait(&bars->full[kb], ti & 1);
@@ -457,13 +510,15 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
   // descales (reference cutlass_mla.py: q_scale * k_scale folded into the softmax scale, k_scale into the output)
   const float sl2 = sm_scale * 1.4426950408889634f * (kv_fp8 ? descale_k * (q_fp8 ? descale_q : 1.f) : 1.f);
   const float osc = kv_fp8 ? descale_k : 1.f;
-  auto kern = q_len == 1 ? (!kv_fp8 ? mla_decode_tc_kernel<false, false, false> : mla_decode_tc_kernel<true, false, false>)
-                         : (!kv_fp8 ? mla_decode_tc_kernel<false, true, false> : mla_decode_tc_kernel<true, true, false>);
+  auto kern = q_len == 1 ? (!kv_fp8 ? mla_decode_tc_kernel<false, false, false, false>
+                                    : mla_decode_tc_kernel<true, false, false, false>)
+                         : (!kv_fp8 ? mla_decode_tc_kernel<false, true, false, false>
+                                    : mla_decode_tc_kernel<true, true, false, false>);
   const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc)");
   if (rc) return rc;
   kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size, max_pages, sl2, num_splits,
                                             part_o, part_ml, kv_fp8 ? q_fp8 : 0, kv_fp8 ? osc : 1.f, tpc, q_len, Qg,
-                                            nullptr, nullptr, 0);
+                                            nullptr, nullptr, 0, Dsv4Keys{});
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc launch");
@@ -479,14 +534,36 @@ int launch_mla_sparse_tc(cudaStream_t st, const void* q_nope, const void* q_pe, 
   const int tiles = (topk + MLA_TOK - 1) / MLA_TOK;
   const int tpc = (tiles + num_splits - 1) / num_splits;
   const float sl2 = sm_scale * 1.4426950408889634f;
-  auto kern = kv_ds_mla ? mla_decode_tc_kernel<true, false, true> : mla_decode_tc_kernel<false, false, true>;
+  auto kern = kv_ds_mla ? mla_decode_tc_kernel<true, false, true, false> : mla_decode_tc_kernel<false, false, true, false>;
   const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc sparse)");
   if (rc) return rc;
   kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, nullptr, page_table, Hq, page_size, max_pages, sl2, num_splits,
-                                            part_o, part_ml, 0, 1.f, tpc, 1, 1, topk_idx, req_id, topk);
+                                            part_o, part_ml, 0, 1.f, tpc, 1, 1, topk_idx, req_id, topk, Dsv4Keys{});
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc sparse launch");
+  return 0;
+}
+
+// DeepSeek-V4 sparse decode: one CTA row (grid.z) per query token over the concatenated main || extra list
+int launch_dsv4_sparse_tc(cudaStream_t st, const void* q, const void* swa_kv, int swa_block, int swa_blocks,
+                          int64_t swa_stride, const int32_t* swa_idx, int swa_topk, const int32_t* swa_lens,
+                          const void* extra_kv, int extra_block, int extra_blocks, int64_t extra_stride,
+                          const int32_t* extra_idx, int extra_topk, const int32_t* extra_lens, int num_tokens, int Hq,
+                          float sm_scale, int num_splits, float* part_o, float* part_ml) {
+  dim3 grid(num_splits, MLA_PARTS, num_tokens);
+  const int tiles = (swa_topk + (extra_idx ? extra_topk : 0) + MLA_TOK - 1) / MLA_TOK;
+  const int tpc = (tiles + num_splits - 1) / num_splits;
+  const float sl2 = sm_scale * 1.4426950408889634f;
+  auto kern = mla_decode_tc_kernel<true, false, true, true>;
+  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc dsv4)");
+  if (rc) return rc;
+  const Dsv4Keys v4{extra_kv, extra_idx, extra_lens, extra_topk, extra_block, extra_blocks, swa_stride, extra_stride};
+  kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q, q, swa_kv, swa_lens, nullptr, Hq, swa_block, swa_blocks, sl2, num_splits,
+                                            part_o, part_ml, 0, 1.f, tpc, 1, 1, swa_idx, nullptr, swa_topk, v4);
+  ++g_launches;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc dsv4 launch");
   return 0;
 }
 

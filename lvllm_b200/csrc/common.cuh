@@ -223,4 +223,11 @@ __host__ __device__ inline uint32_t sw128_offset(uint32_t r, uint32_t b) {
   return (r >> 3) * 1024u + (r & 7u) * 128u + ((((b >> 4) ^ (r & 7u)) & 7u) << 4) + (b & 15u);
 }
 
+// smallest power of two >= x for a positive normal float, from the exponent bits (the reference's exp2(ceil(log2(x))) of
+// the ue8m0 scale format, without the rounding of an fp32 log2 just above a power of two)
+B200_DEVICE float ue8m0_ceil(float x) {
+  const uint32_t b = __float_as_uint(x);
+  return __uint_as_float(((b >> 23) + ((b & 0x7FFFFFu) ? 1u : 0u)) << 23);
+}
+
 }  // namespace b200

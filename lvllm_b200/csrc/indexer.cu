@@ -33,13 +33,6 @@ constexpr int IDX_ROW = 132;    // cache bytes per token: 128 e4m3 + one fp32 sc
 
 B200_DEVICE float bf16r(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
-// smallest power of two >= x for a positive normal float, from the exponent bits (the reference's exp2(ceil(log2(x))) of
-// the ue8m0 scale format, without the rounding of an fp32 log2 just above a power of two)
-B200_DEVICE float ue8m0_ceil(float x) {
-  const uint32_t b = __float_as_uint(x);
-  return __uint_as_float(((b >> 23) + ((b & 0x7FFFFFu) ? 1u : 0u)) << 23);
-}
-
 B200_DEVICE uint32_t e4m3x4(float a, float b, float c, float d) {
   const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
   const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, __NV_E4M3);

@@ -7,7 +7,10 @@
 //                           (cache_kernels.cu:496-590): 512 e4m3 | four fp32 scales, one per 128 dims | 64 bf16 rope dims;
 //   mla_absorb_kernel       ql_nope = q_nope x W_UK^T per head (mla_attention.py:875-893; torch.bmm in the reference);
 //   mla_merge_vup_kernel    the split merge of the decode kernel fused with the v up-projection (mla_attention.py:1154-1176):
-//                           the merged [512] latent output of a (request, head) never leaves shared memory.
+//                           the merged [512] latent output of a (request, head) never leaves shared memory;
+//   dsv4_qnorm_rope_kv_insert_kernel  DeepSeek-V4: q per-head RMSNorm (no weight) + GPT-J RoPE of the last 64 dims, and kv
+//                           RoPE + ue8m0 e4m3 quantisation + insert into the 584-byte cache, in one launch (reference
+//                           csrc/libtorch_stable/fused_deepseek_v4_qnorm_rope_kv_insert_kernel.cu:179-379).
 // All three are HBM / latency bound (W_UK_T and W_UV are 16.8 MB each for 128 heads): coalesced 16-byte loads, every
 // load of a thread's work issued before the first use, fp32 accumulation in a fixed order (deterministic).
 #include <math_constants.h>
@@ -241,6 +244,110 @@ __global__ void __launch_bounds__(512)
   }
 }
 
+// grid = tokens, 256 threads.  Warp w takes the head slots w, w + 8, ... of [0, Hp]: slot h < Hq is query head h, Hq <= h < Hp a
+// padded head (written as zeros) and Hp the token's kv row.  Lane l holds dims [16l, 16l + 16); lanes 28-31 the 64 rope dims.
+//   q:  x * rsqrt(mean(x^2) + eps), then the rope pairs (2p, 2p+1) rotated by (cos, sin)[pos][p]; fp32 throughout, rounded to
+//       bf16 once, into q_out [T, Hp, 512].
+//   kv: the rope pairs rotated, every value rounded to bf16; NoPE dims [64g, 64g + 64) (one quad of lanes) quantised with
+//       scale = 2^ceil(log2(max(amax, 1e-4) / 448)), byte e4m3(x / scale) (saturating) and ue8m0 byte log2(scale) + 127;
+//       row slot_mapping[t] of the cache (block slot / block_size, position slot % block_size, blocks block_stride bytes
+//       apart): 448 e4m3 | 64 bf16 rope at pos * 576, the 7 scale bytes and a zero pad byte at block_size * 576 + pos * 8.
+//       A slot < 0 or past the cache writes nothing.
+__global__ void __launch_bounds__(256)
+    dsv4_qnorm_rope_kv_insert_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kv,
+                                     const int64_t* __restrict__ positions, const float* __restrict__ cos_sin, int max_pos,
+                                     const int64_t* __restrict__ slot_mapping, uint8_t* __restrict__ cache, int block_size,
+                                     int num_blocks, int64_t block_stride, __nv_bfloat16* __restrict__ q_out, int Hq, int Hp,
+                                     float eps) {
+  const int t = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int d0 = lane * 16;
+  const bool rope = d0 >= 448;
+  int64_t pos = positions[t];
+  pos = pos < 0 ? 0 : (pos >= max_pos ? max_pos - 1 : pos);
+  float cs[8], sn[8];
+  if (rope) {
+#pragma unroll
+    for (int p = 0; p < 8; ++p) {
+      cs[p] = cos_sin[pos * 64 + (d0 - 448) / 2 + p];
+      sn[p] = cos_sin[pos * 64 + 32 + (d0 - 448) / 2 + p];
+    }
+  }
+  for (int h = warp; h <= Hp; h += 8) {
+    const bool is_kv = h == Hp;
+    __nv_bfloat16* qo = q_out + ((size_t)t * Hp + h) * 512 + d0;
+    if (!is_kv && h >= Hq) {
+      *reinterpret_cast<uint4*>(qo) = make_uint4(0u, 0u, 0u, 0u);
+      *reinterpret_cast<uint4*>(qo + 8) = make_uint4(0u, 0u, 0u, 0u);
+      continue;
+    }
+    const int64_t slot = is_kv ? slot_mapping[t] : 0;
+    if (is_kv && (slot < 0 || slot >= (int64_t)num_blocks * block_size)) continue;
+    const __nv_bfloat16* src = is_kv ? kv + (size_t)t * 512 + d0 : q + ((size_t)t * Hq + h) * 512 + d0;
+    uint4 raw[2] = {*reinterpret_cast<const uint4*>(src), *reinterpret_cast<const uint4*>(src + 8)};
+    const __nv_bfloat16* hv = reinterpret_cast<const __nv_bfloat16*>(raw);
+    float x[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) x[i] = bf(hv[i]);
+    if (!is_kv) {
+      float ss = 0.f;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) ss = fmaf(x[i], x[i], ss);
+      ss = warp_sum(ss);
+      const float r = rsqrtf(ss / 512.f + eps);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) x[i] *= r;
+    }
+    if (rope) {
+#pragma unroll
+      for (int p = 0; p < 8; ++p) {
+        const float e = x[2 * p], o = x[2 * p + 1];
+        x[2 * p] = fmaf(e, cs[p], -(o * sn[p]));
+        x[2 * p + 1] = fmaf(e, sn[p], o * cs[p]);
+      }
+    }
+    uint32_t pk[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const __nv_bfloat162 b2 = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
+      pk[i] = *reinterpret_cast<const uint32_t*>(&b2);
+    }
+    if (!is_kv) {
+      *reinterpret_cast<uint4*>(qo) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+      *reinterpret_cast<uint4*>(qo + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+      continue;
+    }
+    uint8_t* blk = cache + (size_t)(slot / block_size) * (size_t)block_stride;
+    const int p_in = (int)(slot % block_size);
+    uint8_t* row = blk + (size_t)p_in * 576;
+    if (rope) {
+      *reinterpret_cast<uint4*>(row + 448 + (d0 - 448) * 2) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+      *reinterpret_cast<uint4*>(row + 448 + (d0 - 448) * 2 + 16) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+    }
+    // NoPE values are bf16 already: the quantised block is a quad of lanes
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) amax = fmaxf(amax, fabsf(x[i]));
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+    if (!rope) {
+      const uint32_t e = __float_as_uint(ue8m0_ceil(__fdiv_rn(fmaxf(amax, 1e-4f), 448.f))) >> 23;   // ue8m0 byte
+      const float inv = __uint_as_float((254u - e) << 23);                                            // 1 / scale, exact
+      uint32_t o[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i] * inv, x[4 * i + 1] * inv), __NV_SATFINITE, __NV_E4M3);
+        const uint32_t hi =
+            __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i + 2] * inv, x[4 * i + 3] * inv), __NV_SATFINITE, __NV_E4M3);
+        o[i] = lo | (hi << 16);
+      }
+      *reinterpret_cast<uint4*>(row + d0) = make_uint4(o[0], o[1], o[2], o[3]);
+      uint8_t* srec = blk + (size_t)block_size * 576 + (size_t)p_in * 8;
+      if ((lane & 3) == 0) srec[lane >> 2] = (uint8_t)e;
+      if (lane == 0) srec[7] = 0;
+    }
+  }
+}
+
 void launch_mla_merge_vup(cudaStream_t st, const float* part_o, const float* part_ml, int rows, int num_splits, int Hq,
                           const void* w_uv, void* out_v, void* out_latent, float* lse) {
   mla_merge_vup_kernel<<<rows * Hq, 512, 0, st>>>(part_o, part_ml, num_splits, Hq, reinterpret_cast<const __nv_bfloat16*>(w_uv),
@@ -299,6 +406,30 @@ int b200_mla_decode_vup(void* stream, const void* q_nope, const void* q_pe, int 
   return b200_mla_decode_spec(stream, q_nope, q_pe, q_dtype, kv_cache, kv_dtype, descale_q, descale_k, seq_lens, page_table,
                               batch, 1, num_heads, page_size, max_pages, sm_scale, num_splits, workspace, out_latent, lse,
                               w_uv, out_v);
+}
+
+int b200_dsv4_qnorm_rope_kv_insert(void* stream, const void* q, const void* kv, const int64_t* positions,
+                                   const float* cos_sin_cache, int max_position, const int64_t* slot_mapping, void* cache,
+                                   int block_size, int num_blocks, int64_t block_stride, void* q_out, int num_tokens,
+                                   int num_heads, int q_head_padded, float eps) {
+  auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+  if (!q || !a16(q) || !kv || !a16(kv) || !positions || !cos_sin_cache || (reinterpret_cast<uintptr_t>(cos_sin_cache) & 3u) ||
+      max_position <= 0 || !slot_mapping || !cache || !a16(cache) || block_size <= 0 || num_blocks <= 0 ||
+      block_stride < (int64_t)block_size * 584 || block_stride % 16 != 0 || !q_out || !a16(q_out) || num_tokens < 0 ||
+      num_heads <= 0 || q_head_padded < num_heads || !(eps >= 0.f)) {
+    set_error("b200_dsv4_qnorm_rope_kv_insert: bad argument (16-byte aligned q, kv, cache and q_out, q_head_padded >= "
+              "num_heads, block stride >= block_size * 584 and a multiple of 16)");
+    return B200_ERR_INVALID;
+  }
+  if (num_tokens == 0) return 0;
+  dsv4_qnorm_rope_kv_insert_kernel<<<num_tokens, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(kv), positions, cos_sin_cache,
+      max_position, slot_mapping, reinterpret_cast<uint8_t*>(cache), block_size, num_blocks, block_stride,
+      reinterpret_cast<__nv_bfloat16*>(q_out), num_heads, q_head_padded, eps);
+  ++g_launches;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "dsv4_qnorm_rope_kv_insert launch");
+  return 0;
 }
 
 }  // extern "C"

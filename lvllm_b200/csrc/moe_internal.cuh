@@ -166,6 +166,12 @@ int launch_mla_sparse_tc(cudaStream_t st, const void* q_nope, const void* q_pe, 
                          const int32_t* topk_idx, int topk, const int32_t* req_id, const int32_t* page_table, int max_pages,
                          int num_tokens, int Hq, int page_size, float sm_scale, int num_splits, float* part_o,
                          float* part_ml);
+// DeepSeek-V4 sparse decode over 584-byte caches: main (sliding-window) list || optional extra (compressed) list
+int launch_dsv4_sparse_tc(cudaStream_t st, const void* q, const void* swa_kv, int swa_block, int swa_blocks,
+                          int64_t swa_stride, const int32_t* swa_idx, int swa_topk, const int32_t* swa_lens,
+                          const void* extra_kv, int extra_block, int extra_blocks, int64_t extra_stride,
+                          const int32_t* extra_idx, int extra_topk, const int32_t* extra_lens, int num_tokens, int Hq,
+                          float sm_scale, int num_splits, float* part_o, float* part_ml);
 // split merge of the MLA partials fused with the v up-projection (mla_aux.cu), over rows (b * q_len + i, h)
 void launch_mla_merge_vup(cudaStream_t st, const float* part_o, const float* part_ml, int rows, int num_splits, int Hq,
                           const void* w_uv, void* out_v, void* out_latent, float* lse);

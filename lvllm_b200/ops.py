@@ -283,6 +283,106 @@ def mla_decode_sparse(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_cache: torch.
     return out, lse
 
 
+def _dsv4_cache(c: torch.Tensor, name: str):
+    """(tensor, block_size, num_blocks, block stride in bytes) of a 584-byte-per-token cache, uint8 [blocks, block_size, 584];
+    blocks may be padded (stride(0) > block_size * 584), the bytes of a block are addressed as the per-block layout."""
+    if not c.is_cuda:
+        raise ValueError(f"{name} must be a CUDA tensor (lvllm_b200 has no CPU path)")
+    if c.dtype != torch.uint8 or c.dim() != 3 or c.shape[2] != 584 or c.stride(2) != 1 or c.stride(1) != 584:
+        raise ValueError(f"{name} must be uint8 [blocks, block_size, 584] with rows of 584 contiguous bytes, "
+                         f"got {c.dtype} {tuple(c.shape)} strides {c.stride()}")
+    return c, c.shape[1], c.shape[0], c.stride(0)
+
+
+def dsv4_sparse_decode(q: torch.Tensor, swa_cache: torch.Tensor, swa_indices: torch.Tensor, swa_lens: torch.Tensor,
+                       sm_scale: float, attn_sink: torch.Tensor | None = None, extra_cache: torch.Tensor | None = None,
+                       extra_indices: torch.Tensor | None = None, extra_lens: torch.Tensor | None = None,
+                       num_kv_splits: int = 0) -> torch.Tensor:
+    """Sparse attention decode of DeepSeek-V4 layers (the reference's FlashMLA call with indices, extra_k_cache and attn_sink,
+    models/deepseek_v4/nvidia/flashmla.py:151-244).  q bf16 [T, Hq, 512] (448 NoPE | 64 RoPE dims); the caches are uint8
+    [blocks, block_size, 584] (block layout of flashmla_sparse.py:76-85: block_size x 576 data bytes, then block_size x 8
+    ue8m0 scale bytes).  Token t attends to swa_indices[t, :swa_lens[t]] (global slots of swa_cache) followed by
+    extra_indices[t, :extra_lens[t]] (global slots of extra_cache, compressed layers only); a slot < 0 or past its cache is
+    no key.  One cache row is both key and value.  attn_sink f32 [Hq] adds e^(sink) to each head's softmax denominator.
+    A token with no valid key gets out 0.  Returns out bf16 [T, Hq, 512]."""
+    q = _cuda(q, "q")
+    if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 512:
+        raise ValueError(f"q must be bf16 [tokens, heads, 512], got {q.dtype} {tuple(q.shape)}")
+    T, Hq, _ = q.shape
+    if not 1 <= Hq <= 128 or not 1 <= T <= 65535:
+        raise ValueError(f"dsv4 sparse decode takes 1-128 heads and 1-65535 tokens, got {Hq} heads, {T} tokens")
+    sc, sbs, snb, sstride = _dsv4_cache(swa_cache, "swa_cache")
+
+    def _lists(idx, lens, name):
+        idx = _cuda(idx.to(torch.int32), f"{name}_indices")
+        lens = _cuda(lens.reshape(-1).to(torch.int32), f"{name}_lens")
+        if idx.dim() != 2 or idx.shape[0] != T or idx.shape[1] < 1 or lens.numel() != T:
+            raise ValueError(f"{name}_indices must be [{T}, topk >= 1] and {name}_lens [{T}], got {tuple(idx.shape)} / "
+                             f"{tuple(lens.shape)}")
+        return idx, lens
+
+    si, sl = _lists(swa_indices, swa_lens, "swa")
+    if (extra_cache is None) != (extra_indices is None) or (extra_indices is None) != (extra_lens is None):
+        raise ValueError("extra_cache, extra_indices and extra_lens go together")
+    if extra_cache is not None:
+        ec, ebs, enb, estride = _dsv4_cache(extra_cache, "extra_cache")
+        ei, el = _lists(extra_indices, extra_lens, "extra")
+    else:
+        ec, ebs, enb, estride, ei, el = None, 0, 0, 0, None, None
+    sink = None
+    if attn_sink is not None:
+        sink = _cuda(attn_sink.reshape(-1).to(torch.float32), "attn_sink")
+        if sink.numel() != Hq:
+            raise ValueError(f"attn_sink must hold one value per head ({Hq}), got {sink.numel()}")
+    if num_kv_splits <= 0:
+        # as ops.mla_decode_sparse: a CTA = (token, split, value-dim quarter) walks ceil(tiles / splits) 128-entry tiles of
+        # the concatenated index list; enough splits to fill ~2 waves of the 132 SMs
+        tiles = -(-(si.shape[1] + (ei.shape[1] if ei is not None else 0)) // 128)
+        num_kv_splits = max(1, min(tiles, 264 // (4 * T)))
+    ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(T, Hq, num_kv_splits), dtype=torch.uint8, device=q.device)
+    out = torch.empty(T, Hq, 512, dtype=torch.bfloat16, device=q.device)
+    rc = L.lib().b200_dsv4_sparse_decode(
+        _stream(), q.data_ptr(), T, Hq, sc.data_ptr(), sbs, snb, sstride, si.data_ptr(), si.shape[1], sl.data_ptr(),
+        ec.data_ptr() if ec is not None else None, ebs, enb, estride, ei.data_ptr() if ei is not None else None,
+        ei.shape[1] if ei is not None else 0, el.data_ptr() if el is not None else None,
+        sink.data_ptr() if sink is not None else None, float(sm_scale), int(num_kv_splits), ws.data_ptr(), out.data_ptr())
+    L.check(rc, "b200_dsv4_sparse_decode")
+    return out
+
+
+def dsv4_qnorm_rope_kv_insert(q: torch.Tensor, kv: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.Tensor,
+                              slot_mapping: torch.Tensor, swa_cache: torch.Tensor, q_head_padded: int,
+                              eps: float) -> torch.Tensor:
+    """DeepSeek-V4 q-norm + RoPE + cache insert in one launch (the reference's
+    fused_deepseek_v4_qnorm_rope_kv_rope_quant_insert).  q bf16 [T, Hq, 512] gets a per-head RMSNorm without weight and GPT-J
+    pair RoPE of its last 64 dims (fp32, rounded to bf16 once); kv bf16 [T, 512] (after kv_norm) gets the RoPE, its 448 NoPE
+    dims are quantised per 64 to e4m3 with a ue8m0 scale, and the row goes to slot_mapping[t] of swa_cache (uint8
+    [blocks, block_size, 584]; a slot < 0 writes nothing).  positions int64 [T]; cos_sin_cache f32 [max_pos, 64] = cos | sin.
+    Returns q_out bf16 [T, q_head_padded, 512], heads past Hq zero."""
+    q, kv = _cuda(q, "q"), _cuda(kv, "kv")
+    if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 512:
+        raise ValueError(f"q must be bf16 [tokens, heads, 512], got {q.dtype} {tuple(q.shape)}")
+    T, Hq, _ = q.shape
+    if kv.dtype != torch.bfloat16 or tuple(kv.shape) != (T, 512):
+        raise ValueError(f"kv must be bf16 [{T}, 512], got {kv.dtype} {tuple(kv.shape)}")
+    if int(q_head_padded) < Hq:
+        raise ValueError(f"q_head_padded ({q_head_padded}) must be >= the head count ({Hq})")
+    cs = _cuda(cos_sin_cache, "cos_sin_cache")
+    if cs.dtype != torch.float32 or cs.dim() != 2 or cs.shape[1] != 64:
+        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cs.dtype} {tuple(cs.shape)}")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    slots = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
+    if pos.numel() != T or slots.numel() != T:
+        raise ValueError(f"positions and slot_mapping need one entry per token ({T})")
+    c, bs, nb, stride = _dsv4_cache(swa_cache, "swa_cache")
+    q_out = torch.empty(T, int(q_head_padded), 512, dtype=torch.bfloat16, device=q.device)
+    rc = L.lib().b200_dsv4_qnorm_rope_kv_insert(_stream(), q.data_ptr(), kv.data_ptr(), pos.data_ptr(), cs.data_ptr(),
+                                                cs.shape[0], slots.data_ptr(), c.data_ptr(), bs, nb, stride, q_out.data_ptr(),
+                                                T, Hq, int(q_head_padded), float(eps))
+    L.check(rc, "b200_dsv4_qnorm_rope_kv_insert")
+    return q_out
+
+
 def mla_rope_cache_write(q_pe: torch.Tensor, k_pe: torch.Tensor, kv_c: torch.Tensor, positions: torch.Tensor,
                          cos_sin_cache: torch.Tensor, slot_mapping: torch.Tensor, kv_cache: torch.Tensor,
                          is_neox_style: bool = False, kv_scale: float = 1.0) -> None:
