@@ -228,18 +228,30 @@ __global__ void __launch_bounds__(128) mla_merge_kernel(const float* __restrict_
   if (lse && tid == 0) lse[w] = (lsum > 0.f) ? (mx * 0.6931471805599453f + logf(lsum)) : -CUDART_INF_F;
 }
 
+// split partials of the MLA-family decode kernel in the workspace: O [rows * num_heads * num_splits][512], then (m, l)
+struct MlaPartials {
+  float *o, *ml;
+};
+static MlaPartials mla_partials(void* workspace, int rows, int num_heads, int num_splits) {
+  float* po = reinterpret_cast<float*>(workspace);
+  return {po, po + (size_t)rows * num_heads * num_splits * 512};
+}
+
 // merge of the MLA decode kernel's partials over query rows x heads: fused with the v up-projection when w_uv is given
-// (mla_aux.cu), mla_merge_kernel up to 512 splits, decode_merge_kernel above
-static int mla_merge(cudaStream_t st, const float* po, const float* pml, int rows, int num_heads, int num_splits, void* out,
-                     float* lse, const void* w_uv, void* out_v) {
+// (mla_aux.cu), mla_merge_kernel up to 512 splits (with the DeepSeek-V4 attention sink when sink is given),
+// decode_merge_kernel above.  The fused v up-projection has no sink: the two are exclusive.
+static int mla_merge(cudaStream_t st, const MlaPartials& p, int rows, int num_heads, int num_splits, void* out, float* lse,
+                     const void* w_uv, void* out_v, const float* sink = nullptr) {
+  const float *po = p.o, *pml = p.ml;
+  auto bo = reinterpret_cast<__nv_bfloat16*>(out);
   if (w_uv)
     launch_mla_merge_vup(st, po, pml, rows, num_splits, num_heads, w_uv, out_v, out, lse);
+  else if (sink)
+    mla_merge_kernel<true><<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, bo, lse, sink, num_heads);
   else if (num_splits <= 512)
-    mla_merge_kernel<false><<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, reinterpret_cast<__nv_bfloat16*>(out), lse,
-                                                             nullptr, num_heads);
+    mla_merge_kernel<false><<<rows * num_heads, 128, 0, st>>>(po, pml, num_splits, bo, lse, nullptr, num_heads);
   else
-    decode_merge_kernel<512><<<(rows * num_heads + 3) / 4, 128, 0, st>>>(po, pml, rows * num_heads, num_splits,
-                                                                        reinterpret_cast<__nv_bfloat16*>(out), lse);
+    decode_merge_kernel<512><<<(rows * num_heads + 3) / 4, 128, 0, st>>>(po, pml, rows * num_heads, num_splits, bo, lse);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "mla merge launch");
@@ -292,13 +304,12 @@ int b200_mla_decode_spec(void* stream, const void* q_nope, const void* q_pe, int
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int rows = batch * q_len;   // query rows (b, i), b * q_len + i
-  float* po = reinterpret_cast<float*>(workspace);
-  float* pml = po + (size_t)rows * num_heads * num_splits * 512;
+  const MlaPartials p = mla_partials(workspace, rows, num_heads, num_splits);
   // each CTA walks ceil(tiles / num_splits) 128-token tiles (online softmax)
   int rc = launch_mla_tc(st, q_nope, q_pe, kv_cache, seq_lens, page_table, batch, q_len, num_heads, page_size, max_pages,
-                         sm_scale, num_splits, po, pml, kv_dtype, q_dtype, descale_q, descale_k);
+                         sm_scale, num_splits, p.o, p.ml, kv_dtype, q_dtype, descale_q, descale_k);
   if (rc) return rc;
-  return mla_merge(st, po, pml, rows, num_heads, num_splits, out, lse, w_uv, out_v);
+  return mla_merge(st, p, rows, num_heads, num_splits, out, lse, w_uv, out_v);
 }
 
 int b200_mla_decode_sparse(void* stream, const void* q_nope, const void* q_pe, const void* kv_cache, int kv_dtype,
@@ -313,12 +324,11 @@ int b200_mla_decode_sparse(void* stream, const void* q_nope, const void* q_pe, c
     return B200_ERR_INVALID;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  float* po = reinterpret_cast<float*>(workspace);
-  float* pml = po + (size_t)num_tokens * num_heads * num_splits * 512;
+  const MlaPartials p = mla_partials(workspace, num_tokens, num_heads, num_splits);
   const int rc = launch_mla_sparse_tc(st, q_nope, q_pe, kv_cache, kv_dtype == 2, topk_indices, topk, req_id, page_table,
-                                      max_pages, num_tokens, num_heads, page_size, sm_scale, num_splits, po, pml);
+                                      max_pages, num_tokens, num_heads, page_size, sm_scale, num_splits, p.o, p.ml);
   if (rc) return rc;
-  return mla_merge(st, po, pml, num_tokens, num_heads, num_splits, out, lse, w_uv, out_v);
+  return mla_merge(st, p, num_tokens, num_heads, num_splits, out, lse, w_uv, out_v);
 }
 
 int b200_dsv4_sparse_decode(void* stream, const void* q, int num_tokens, int num_heads, const void* swa_cache,
@@ -347,22 +357,13 @@ int b200_dsv4_sparse_decode(void* stream, const void* q, int num_tokens, int num
     return B200_ERR_INVALID;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  float* po = reinterpret_cast<float*>(workspace);
-  float* pml = po + (size_t)num_tokens * num_heads * num_splits * 512;
+  const MlaPartials p = mla_partials(workspace, num_tokens, num_heads, num_splits);
   int rc = launch_dsv4_sparse_tc(st, q, swa_cache, swa_block_size, swa_num_blocks, swa_block_stride, swa_indices, swa_topk,
                                  swa_lens, extra_cache, extra_block_size, extra_num_blocks, extra_block_stride,
                                  extra ? extra_indices : nullptr, extra_topk, extra_lens, num_tokens, num_heads, sm_scale,
-                                 num_splits, po, pml);
+                                 num_splits, p.o, p.ml);
   if (rc) return rc;
-  auto bo = reinterpret_cast<__nv_bfloat16*>(out);
-  if (attn_sink)
-    mla_merge_kernel<true><<<num_tokens * num_heads, 128, 0, st>>>(po, pml, num_splits, bo, nullptr, attn_sink, num_heads);
-  else
-    mla_merge_kernel<false><<<num_tokens * num_heads, 128, 0, st>>>(po, pml, num_splits, bo, nullptr, nullptr, num_heads);
-  ++g_launches;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "dsv4 merge launch");
-  return 0;
+  return mla_merge(st, p, num_tokens, num_heads, num_splits, out, nullptr, nullptr, nullptr, attn_sink);
 }
 
 int b200_gqa_decode(void* stream, const void* q, const void* k_cache, const void* v_cache, const int32_t* seq_lens,

@@ -277,87 +277,77 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
         }
       }
       }
-      if (KV8) {
-        // e4m3 cache (and, with q8, e4m3 queries): 8-byte loads, widened to bf16 in registers, 16-byte stores into the
-        // swizzled tiles; MLA_PF k-blocks of loads are kept in flight per thread (register ring)
-        constexpr int MLA_PF = 3;
-        uint2 kreg[MLA_PF][8], qreg[MLA_PF][8];
-        auto issue = [&](int j, int buf) {
-          const int kb = kb_of(j);
+      // KV8: e4m3 cache (and, with q8, e4m3 queries): 8-byte loads, widened to bf16 in registers, 16-byte stores into the
+      // swizzled tiles; MLA_PF k-blocks of loads are kept in flight per thread (register ring).  Otherwise every block goes
+      // in by cp.async (LDGSTS) straight into the swizzled tiles, with no register staging.
+      constexpr int MLA_PF = KV8 ? 3 : 1;
+      uint2 kreg[MLA_PF][8], qreg[MLA_PF][8];
+      auto issue = [&](int j, int buf) {
+        const int kb = kb_of(j);
 #pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const int r = r0 + 16 * u;
-            // fp8_ds_mla: the rope block (kb 8, V4: kb 7) is bf16 and goes in by cp.async
-            kreg[buf][u] = krow8[u] && !(SPARSE && kb == ROPE_KB)
-                               ? __ldg(reinterpret_cast<const uint2*>(krow8[u] + kb * 64 + c * 8)) : make_uint2(0u, 0u);
-            qreg[buf][u] = make_uint2(0u, 0u);
-            if (!SPARSE && q8 && r < nrows)
-              qreg[buf][u] = __ldg(reinterpret_cast<const uint2*>(kb < 8 ? qn8 + (row0 + r) * 512 + kb * 64 + c * 8
-                                                                           : qp8 + (row0 + r) * 64 + c * 8));
-          }
-        };
-#pragma unroll
-        for (int j = 0; j < MLA_PF - 1; ++j) issue(j, j);
-#pragma unroll
-        for (int j = 0; j < KB; ++j, ++qit) {
-          const int kb = kb_of(j);
-          const int s = qit % MLA_QSTAGES, buf = j % MLA_PF;
-          if (j + MLA_PF - 1 < KB) issue(j + MLA_PF - 1, (j + MLA_PF - 1) % MLA_PF);
-          if (ti > 0) mla_wait(j < MLA_NO ? &bars->s_full : &bars->o_full, (ti - 1) & 1);   // the block's previous readers are done
-          if (SPARSE && j == 0 && lane == 0) {   // publish the mask once tile ti - 1's QK^T is done (see v_full)
-            bars->kvalid[ti & 1][warp - 8] = vword;
-            mbar_arrive(&bars->v_full);
-          }
-          mla_wait(&bars->empty[s], ((qit / MLA_QSTAGES) & 1) ^ 1);
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const int r = r0 + 16 * u;
-            if (!SPARSE && q8) {
-              *reinterpret_cast<uint4*>(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(qreg[buf][u]);
-            } else {
-              const bool qok = r < nrows;
-              const __nv_bfloat16* qsrc = !qok ? q_nope
-                                               : (kb < 8 ? q_nope + (row0 + r) * 512 + kb * 64 + c * 8
-                                                         : q_pe + (row0 + r) * 64 + c * 8);
-              cp_async16(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16), qsrc, qok);
-            }
-            if (!SPARSE)
-              *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(kreg[buf][u]);
-            else if (kb < ROPE_KB)
-              *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) =
-                  fp8x8_scaled_to_bf16x8(kreg[buf][u], V4 ? ue8m0_scale(kue[u], kb) : kscale[u][kb >> 1]);
-            else
-              cp_async16(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16),
-                         krow8[u] ? krow8[u] + (V4 ? 448 : 528) + c * 16 : kv_v, krow8[u] != nullptr);
-          }
-          if (SPARSE || !q8) asm volatile("cp.async.wait_all;" ::: "memory");
-          fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
-          mbar_arrive(&bars->full[kb]);
+        for (int u = 0; u < 8; ++u) {
+          const int r = r0 + 16 * u;
+          // fp8_ds_mla: the rope block (kb 8, V4: kb 7) is bf16 and goes in by cp.async
+          kreg[buf][u] = krow8[u] && !(SPARSE && kb == ROPE_KB)
+                             ? __ldg(reinterpret_cast<const uint2*>(krow8[u] + kb * 64 + c * 8)) : make_uint2(0u, 0u);
+          qreg[buf][u] = make_uint2(0u, 0u);
+          if (!SPARSE && q8 && r < nrows)
+            qreg[buf][u] = __ldg(reinterpret_cast<const uint2*>(kb < 8 ? qn8 + (row0 + r) * 512 + kb * 64 + c * 8
+                                                                         : qp8 + (row0 + r) * 64 + c * 8));
         }
-      } else {
-        // cp.async (LDGSTS) straight into the swizzled tiles: no register staging; completion is signalled per k-block
-        for (int j = 0; j < KB; ++j, ++qit) {
-          const int kb = kb_of(j);
-          const int s = qit % MLA_QSTAGES;
-          if (ti > 0) mla_wait(j < MLA_NO ? &bars->s_full : &bars->o_full, (ti - 1) & 1);
-          if (SPARSE && j == 0 && lane == 0) {   // publish the mask once tile ti - 1's QK^T is done (see v_full)
-            bars->kvalid[ti & 1][warp - 8] = vword;
-            mbar_arrive(&bars->v_full);
-          }
-          mla_wait(&bars->empty[s], ((qit / MLA_QSTAGES) & 1) ^ 1);
+      };
+      // one k-block per step, the same sequence for every key source and cache format: wait until the block's previous
+      // readers are done, (SPARSE) publish the tile's mask, wait for a q-ring slot, fill q and k, signal full[kb]
+      auto step = [&](int j) {
+        const int kb = kb_of(j);
+        const int s = qit % MLA_QSTAGES, buf = j % MLA_PF;
+        if (KV8 && j + MLA_PF - 1 < KB) issue(j + MLA_PF - 1, (j + MLA_PF - 1) % MLA_PF);
+        if (ti > 0) mla_wait(j < MLA_NO ? &bars->s_full : &bars->o_full, (ti - 1) & 1);
+        if (SPARSE && j == 0 && lane == 0) {   // publish the mask once tile ti - 1's QK^T is done (see v_full)
+          bars->kvalid[ti & 1][warp - 8] = vword;
+          mbar_arrive(&bars->v_full);
+        }
+        mla_wait(&bars->empty[s], ((qit / MLA_QSTAGES) & 1) ^ 1);
 #pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const int r = r0 + 16 * u;
+        for (int u = 0; u < 8; ++u) {
+          const int r = r0 + 16 * u;
+          if (KV8 && !SPARSE && q8) {
+            *reinterpret_cast<uint4*>(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(qreg[buf][u]);
+          } else {
             const bool qok = r < nrows;
             const __nv_bfloat16* qsrc = !qok ? q_nope
                                              : (kb < 8 ? q_nope + (row0 + r) * 512 + kb * 64 + c * 8
                                                        : q_pe + (row0 + r) * 64 + c * 8);
             cp_async16(q_ring + s * TILE_BYTES + sw128_offset(r, c * 16), qsrc, qok);
-            const bool kok = krow[u] != nullptr;
-            cp_async16(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16), kok ? krow[u] + kb * 64 + c * 8 : kv, kok);
           }
-          cp_async_mbar_arrive_noinc(&bars->full[kb]);
+          if (!KV8)
+            cp_async16(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16), krow[u] ? krow[u] + kb * 64 + c * 8 : kv,
+                       krow[u] != nullptr);
+          else if (!SPARSE)
+            *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) = fp8x8_to_bf16x8(kreg[buf][u]);
+          else if (kb < ROPE_KB)
+            *reinterpret_cast<uint4*>(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16)) =
+                fp8x8_scaled_to_bf16x8(kreg[buf][u], V4 ? ue8m0_scale(kue[u], kb) : kscale[u][kb >> 1]);
+          else
+            cp_async16(k_area + kb * TILE_BYTES + sw128_offset(r, c * 16),
+                       krow8[u] ? krow8[u] + (V4 ? 448 : 528) + c * 16 : kv_v, krow8[u] != nullptr);
         }
+        if (!KV8) {
+          cp_async_mbar_arrive_noinc(&bars->full[kb]);   // arrives when this thread's cp.async writes have landed
+        } else {
+          if (SPARSE || !q8) asm volatile("cp.async.wait_all;" ::: "memory");
+          fence_proxy_async();   // generic-proxy stores -> wgmma (async proxy) reads
+          mbar_arrive(&bars->full[kb]);
+        }
+      };
+      // the register ring needs the k-block loop unrolled; the cp.async loop stays rolled
+      if (KV8) {
+#pragma unroll
+        for (int j = 0; j < MLA_PF - 1; ++j) issue(j, j);
+#pragma unroll
+        for (int j = 0; j < KB; ++j, ++qit) step(j);
+      } else {
+        for (int j = 0; j < KB; ++j, ++qit) step(j);
       }
     }
   } else {
@@ -494,6 +484,23 @@ __global__ void __launch_bounds__(MLA_THREADS, 1)
   }
 }
 
+// each CTA walks ceil(tiles / num_splits) of the ceil(max_keys / 128) key tiles with an online softmax
+static int tiles_per_cta(int64_t max_keys, int num_splits) {
+  const int tiles = (int)((max_keys + MLA_TOK - 1) / MLA_TOK);
+  return (tiles + num_splits - 1) / num_splits;
+}
+// the tail every MLA-family launch shares: raise the kernel's dynamic shared memory, launch, check
+template <class Kern, class... Args>
+static int launch_mla(Kern kern, dim3 grid, cudaStream_t st, Args... args) {
+  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc)");
+  if (rc) return rc;
+  kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(args...);
+  ++g_launches;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc launch");
+  return 0;
+}
+
 int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const void* kv, const int32_t* seq_lens,
                   const int32_t* page_table, int batch, int q_len, int Hq, int page_size, int max_pages, float sm_scale,
                   int num_splits, float* part_o, float* part_ml, int kv_fp8, int q_fp8, float descale_q, float descale_k) {
@@ -504,9 +511,8 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
   // draft tokens per q-group (as many as fill the 128 MMA rows), q-groups; the q-group varies with the part in grid.y
   const int Qg = min(q_len, 128 / Hq), n_qg = (q_len + Qg - 1) / Qg;
   dim3 grid(num_splits, MLA_PARTS * n_qg, batch);
-  // each CTA walks tpc consecutive 128-token tiles (online softmax); the splits together cover the page table
-  const int tiles = (int)(((int64_t)max_pages * page_size + MLA_TOK - 1) / MLA_TOK);
-  const int tpc = (tiles + num_splits - 1) / num_splits;
+  // the splits together cover the page table
+  const int tpc = tiles_per_cta((int64_t)max_pages * page_size, num_splits);
   // descales (reference cutlass_mla.py: q_scale * k_scale folded into the softmax scale, k_scale into the output)
   const float sl2 = sm_scale * 1.4426950408889634f * (kv_fp8 ? descale_k * (q_fp8 ? descale_q : 1.f) : 1.f);
   const float osc = kv_fp8 ? descale_k : 1.f;
@@ -514,15 +520,8 @@ int launch_mla_tc(cudaStream_t st, const void* q_nope, const void* q_pe, const v
                                     : mla_decode_tc_kernel<true, false, false, false>)
                          : (!kv_fp8 ? mla_decode_tc_kernel<false, true, false, false>
                                     : mla_decode_tc_kernel<true, true, false, false>);
-  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc)");
-  if (rc) return rc;
-  kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size, max_pages, sl2, num_splits,
-                                            part_o, part_ml, kv_fp8 ? q_fp8 : 0, kv_fp8 ? osc : 1.f, tpc, q_len, Qg,
-                                            nullptr, nullptr, 0, Dsv4Keys{});
-  ++g_launches;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc launch");
-  return 0;
+  return launch_mla(kern, grid, st, q_nope, q_pe, kv, seq_lens, page_table, Hq, page_size, max_pages, sl2, num_splits, part_o,
+                    part_ml, kv_fp8 ? q_fp8 : 0, kv_fp8 ? osc : 1.f, tpc, q_len, Qg, nullptr, nullptr, 0, Dsv4Keys{});
 }
 
 // sparse decode: one CTA row (grid.z) per query token; kv_ds_mla selects the fp8_ds_mla cache
@@ -531,18 +530,10 @@ int launch_mla_sparse_tc(cudaStream_t st, const void* q_nope, const void* q_pe, 
                          int num_tokens, int Hq, int page_size, float sm_scale, int num_splits, float* part_o,
                          float* part_ml) {
   dim3 grid(num_splits, MLA_PARTS, num_tokens);
-  const int tiles = (topk + MLA_TOK - 1) / MLA_TOK;
-  const int tpc = (tiles + num_splits - 1) / num_splits;
   const float sl2 = sm_scale * 1.4426950408889634f;
   auto kern = kv_ds_mla ? mla_decode_tc_kernel<true, false, true, false> : mla_decode_tc_kernel<false, false, true, false>;
-  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc sparse)");
-  if (rc) return rc;
-  kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q_nope, q_pe, kv, nullptr, page_table, Hq, page_size, max_pages, sl2, num_splits,
-                                            part_o, part_ml, 0, 1.f, tpc, 1, 1, topk_idx, req_id, topk, Dsv4Keys{});
-  ++g_launches;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc sparse launch");
-  return 0;
+  return launch_mla(kern, grid, st, q_nope, q_pe, kv, nullptr, page_table, Hq, page_size, max_pages, sl2, num_splits, part_o,
+                    part_ml, 0, 1.f, tiles_per_cta(topk, num_splits), 1, 1, topk_idx, req_id, topk, Dsv4Keys{});
 }
 
 // DeepSeek-V4 sparse decode: one CTA row (grid.z) per query token over the concatenated main || extra list
@@ -552,19 +543,11 @@ int launch_dsv4_sparse_tc(cudaStream_t st, const void* q, const void* swa_kv, in
                           const int32_t* extra_idx, int extra_topk, const int32_t* extra_lens, int num_tokens, int Hq,
                           float sm_scale, int num_splits, float* part_o, float* part_ml) {
   dim3 grid(num_splits, MLA_PARTS, num_tokens);
-  const int tiles = (swa_topk + (extra_idx ? extra_topk : 0) + MLA_TOK - 1) / MLA_TOK;
-  const int tpc = (tiles + num_splits - 1) / num_splits;
+  const int tpc = tiles_per_cta(swa_topk + (extra_idx ? extra_topk : 0), num_splits);
   const float sl2 = sm_scale * 1.4426950408889634f;
-  auto kern = mla_decode_tc_kernel<true, false, true, true>;
-  const int rc = kernel_smem(reinterpret_cast<const void*>(kern), MLA_SMEM, "cudaFuncSetAttribute(mla_decode_tc dsv4)");
-  if (rc) return rc;
   const Dsv4Keys v4{extra_kv, extra_idx, extra_lens, extra_topk, extra_block, extra_blocks, swa_stride, extra_stride};
-  kern<<<grid, MLA_THREADS, MLA_SMEM, st>>>(q, q, swa_kv, swa_lens, nullptr, Hq, swa_block, swa_blocks, sl2, num_splits,
-                                            part_o, part_ml, 0, 1.f, tpc, 1, 1, swa_idx, nullptr, swa_topk, v4);
-  ++g_launches;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "mla_decode_tc dsv4 launch");
-  return 0;
+  return launch_mla(mla_decode_tc_kernel<true, false, true, true>, grid, st, q, q, swa_kv, swa_lens, nullptr, Hq, swa_block,
+                    swa_blocks, sl2, num_splits, part_o, part_ml, 0, 1.f, tpc, 1, 1, swa_idx, nullptr, swa_topk, v4);
 }
 
 }  // namespace b200

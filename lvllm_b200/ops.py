@@ -173,6 +173,14 @@ def rmsnorm_cast(x_f32: torch.Tensor, out: torch.Tensor, gain: float = 1.0, eps:
     return out
 
 
+def _mla_splits(max_keys: int, rows: int) -> int:
+    """Default split count of the MLA-family decode kernel (mla_decode, mla_decode_sparse, dsv4_sparse_decode).  A CTA =
+    (grid row, split, value-dim quarter) walks ceil(tiles / splits) of the ceil(max_keys / 128) key tiles with an online
+    softmax; rows = grid rows (requests x q-groups, or query tokens).  Enough splits to fill ~2 waves of the 132 SMs, no
+    more: each split costs an fp32 partial of the output."""
+    return max(1, min(-(-max_keys // 128), 264 // (4 * rows)))
+
+
 def mla_decode(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_c_and_k_pe_cache: torch.Tensor, seq_lens: torch.Tensor,
                page_table: torch.Tensor, sm_scale: float, num_kv_splits: int = 0, max_seq_len: int | None = None,
                q_scale: float = 1.0, k_scale: float = 1.0, w_uv: torch.Tensor | None = None, q_len_per_req: int = 1):
@@ -212,12 +220,8 @@ def mla_decode(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_c_and_k_pe_cache: to
         if max_pages != pt.shape[1]:
             pt = pt[:, :max_pages].contiguous()
     if num_kv_splits <= 0:
-        # a CTA = (request, q-group, split, value-dim quarter) walks ceil(tiles / splits) 128-token tiles with an online
-        # softmax: enough splits to fill ~2 waves of the 132 SMs, no more (each split costs an fp32 partial of the output)
-        tiles = max(1, -(-(max_pages * page) // 128))
-        qg = max(1, min(Q, 128 // Hq))   # draft tokens per q-group (the kernel's 128 MMA rows); n_qg q-groups
-        n_qg = -(-Q // qg)
-        num_kv_splits = max(1, min(tiles, 264 // (4 * B * n_qg)))
+        qg = max(1, min(Q, 128 // Hq))   # draft tokens per q-group (the kernel's 128 MMA rows)
+        num_kv_splits = _mla_splits(max_pages * page, B * -(-Q // qg))   # grid rows: requests x q-groups
     ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(T, Hq, num_kv_splits), dtype=torch.uint8, device=qn.device)
     out = torch.empty(T, Hq, 512, dtype=torch.bfloat16, device=qn.device)
     lse = torch.empty(T, Hq, dtype=torch.float32, device=qn.device)
@@ -263,10 +267,7 @@ def mla_decode_sparse(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_cache: torch.
         raise ValueError(f"page_table must be [requests, max_pages], got {tuple(pt.shape)}")
     topk = idx.shape[1]
     if num_kv_splits <= 0:
-        # as ops.mla_decode: a CTA = (token, split, value-dim quarter) walks ceil(tiles / splits) 128-entry index tiles;
-        # enough splits to fill ~2 waves of the 132 SMs
-        tiles = -(-topk // 128)
-        num_kv_splits = max(1, min(tiles, 264 // (4 * T)))
+        num_kv_splits = _mla_splits(topk, T)
     ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(T, Hq, num_kv_splits), dtype=torch.uint8, device=qn.device)
     out = torch.empty(T, Hq, 512, dtype=torch.bfloat16, device=qn.device)
     lse = torch.empty(T, Hq, dtype=torch.float32, device=qn.device)
@@ -335,10 +336,7 @@ def dsv4_sparse_decode(q: torch.Tensor, swa_cache: torch.Tensor, swa_indices: to
         if sink.numel() != Hq:
             raise ValueError(f"attn_sink must hold one value per head ({Hq}), got {sink.numel()}")
     if num_kv_splits <= 0:
-        # as ops.mla_decode_sparse: a CTA = (token, split, value-dim quarter) walks ceil(tiles / splits) 128-entry tiles of
-        # the concatenated index list; enough splits to fill ~2 waves of the 132 SMs
-        tiles = -(-(si.shape[1] + (ei.shape[1] if ei is not None else 0)) // 128)
-        num_kv_splits = max(1, min(tiles, 264 // (4 * T)))
+        num_kv_splits = _mla_splits(si.shape[1] + (ei.shape[1] if ei is not None else 0), T)
     ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(T, Hq, num_kv_splits), dtype=torch.uint8, device=q.device)
     out = torch.empty(T, Hq, 512, dtype=torch.bfloat16, device=q.device)
     rc = L.lib().b200_dsv4_sparse_decode(
