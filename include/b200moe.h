@@ -260,6 +260,39 @@ int b200_dsv4_qnorm_rope_kv_insert(void* stream, const void* q, const void* kv, 
                                    const float* cos_sin_cache, int max_position, const int64_t* slot_mapping, void* cache,
                                    int block_size, int num_blocks, int64_t block_stride, void* q_out, int num_tokens,
                                    int num_heads, int q_head_padded, float eps);
+/* DeepSeek-V4 manifold hyper-connections (mHC) for decode, hc_mult = 4 (the reference's mhc_pre / mhc_post /
+ * mhc_fused_post_pre / hc_head, vllm/model_executor/kernels/mhc/torch.py:6-106, tilelang_kernels.py:305-350, 884-977).
+ * residual bf16 [T, 4, H], x bf16 [T, H], post_layer_mix f32 [T, 4], comb_res_mix f32 [T, 4, 4] (comb[i][j] maps stream i to
+ * stream j), fn f32 [24, 4H] row-major, hc_scale f32 [3], hc_base f32 [24]; norm_weight bf16 [H] or NULL.
+ *   post   r'[t, j] = bf16(post[t, j] x[t] + sum_i comb[t, i, j] residual[t, i]), fp32, rounded once;
+ *   pre    on r (= r' when x is given, else residual), r_flat the fp32 row [4H]:
+ *          mixes = (r_flat . fn^T) * rsqrt(sum r_flat^2 / 4H + rms_eps),
+ *          pre_i = sigmoid(mixes_i s0 + base_i) + hc_pre_eps, post_mix_j = sigmoid(mixes_{4+j} s1 + base_{4+j}) * post_mult,
+ *          comb_mix = sinkhorn(mixes_{8..23} s2 + base_{8..23}) as [4, 4] (row softmax + eps, column normalise, then
+ *          sinkhorn_repeat - 1 times row and column normalisation, each dividing by sum + hc_sinkhorn_eps),
+ *          layer_input = bf16(sum_i pre_i r_i); with norm_weight: the fp32 row o is stored as bf16 and
+ *          layer_input = bf16(float(bf16(o)) * rsqrt(mean(o^2) + norm_eps) * w), the mean square from the unrounded o.
+ * Outputs: residual_out bf16 [T, 4, H] (r'), post_mix f32 [T, 4], comb_mix f32 [T, 4, 4], layer_input bf16 [T, H].
+ * x NULL: pre only, and post_layer_mix, comb_res_mix and residual_out must be NULL.  A token's outputs do not depend on the
+ * other tokens of the batch (the reduction is split by H only), and the fused call gives the bits of b200_mhc_post followed
+ * by the pre-only call.  Workspace: b200_mhc_workspace_bytes(T, H) bytes, 16-byte aligned.  No allocation, no
+ * synchronisation (graph-capturable).  B200_ERR_INVALID, nothing launched: a NULL required pointer, a bf16 tensor, fn or the
+ * workspace not 16-byte aligned, an f32 array not 4-byte aligned, T outside [1, 2^20], H not a multiple of 64 in
+ * [256, 16384], sinkhorn_repeat < 1, a negative (or NaN) eps. */
+int64_t b200_mhc_workspace_bytes(int num_tokens, int hidden_size);   /* = T * (H / 64) * 25 * 4 */
+int b200_mhc_post_pre(void* stream, const void* x, const void* residual, const float* post_layer_mix,
+                      const float* comb_res_mix, const float* fn, const float* hc_scale, const float* hc_base,
+                      const void* norm_weight, int num_tokens, int hidden_size, float rms_eps, float hc_pre_eps,
+                      float hc_sinkhorn_eps, float hc_post_mult_value, int sinkhorn_repeat, float norm_eps,
+                      void* workspace, void* residual_out, float* post_mix, float* comb_mix, void* layer_input);
+/* post alone: out bf16 [T, 4, H] = r' as above (the same expression, the same bits). */
+int b200_mhc_post(void* stream, const void* x, const void* residual, const float* post_layer_mix, const float* comb_res_mix,
+                  int num_tokens, int hidden_size, void* out);
+/* hc_head: fn f32 [4, 4H], hc_scale f32 [1], hc_base f32 [4];
+ * out bf16 [T, H] = bf16(sum_i (sigmoid(mixes_i s0 + base_i) + hc_eps) residual_i), mixes as in the pre step.
+ * Workspace b200_mhc_workspace_bytes(T, H); refusals as b200_mhc_post_pre. */
+int b200_hc_head(void* stream, const void* residual, const float* fn, const float* hc_scale, const float* hc_base,
+                 int num_tokens, int hidden_size, float rms_eps, float hc_eps, void* workspace, void* out);
 /* The MLA decode kernel's neighbours (SURVEY.md 8f row 3), bf16:
  *  b200_mla_rope_cache_write  RoPE of q_pe [T,Hq,64] and k_pe [T,64] in place (rotary_embedding/base.py:161-201; cos_sin_cache
  *      bf16 [max_pos,64] = cos | sin; is_neox 0 = GPT-J pairs (DeepSeek), 1 = NeoX halves) fused with concat_and_cache_mla

@@ -87,6 +87,11 @@ PROTOTYPES = {
                                     _f32, _i32, _vp, _vp, _vp]),
     "b200_gqa_qknorm_rope_cache_write": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _vp, _vp, _i64,
                                                 _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32]),
+    "b200_mhc_workspace_bytes": (_i64, [_i32, _i32]),
+    "b200_mhc_post_pre": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _f32, _f32, _f32, _i32, _f32,
+                                 _vp, _vp, _vp, _vp, _vp]),
+    "b200_mhc_post": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
+    "b200_hc_head": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _f32, _vp, _vp]),
     "b200_ep_flag_bytes": (_i64, []),
     "b200_ep_buffer_create": (_i32, [_i64, C.POINTER(_vp), _vp]),
     "b200_ep_buffer_open": (_i32, [_vp, C.POINTER(_vp)]),

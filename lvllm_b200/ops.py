@@ -381,6 +381,118 @@ def dsv4_qnorm_rope_kv_insert(q: torch.Tensor, kv: torch.Tensor, positions: torc
     return q_out
 
 
+def _mhc_streams(residual: torch.Tensor, name: str = "residual"):
+    """bf16 [..., 4, H] -> (contiguous tensor, leading shape, T, H)."""
+    r = _cuda(residual, name)
+    if r.dtype != torch.bfloat16 or r.dim() < 2 or r.shape[-2] != 4:
+        raise ValueError(f"{name} must be bf16 [..., 4, hidden] (hc_mult = 4), got {r.dtype} {tuple(r.shape)}")
+    lead = tuple(r.shape[:-2])
+    return r, lead, r.numel() // (4 * r.shape[-1]) if r.numel() else 0, r.shape[-1]
+
+
+def _mhc_f32(t: torch.Tensor, numel: int, name: str) -> torch.Tensor:
+    t = _cuda(t.to(torch.float32), name)
+    if t.numel() != numel:
+        raise ValueError(f"{name} must hold {numel} float32 values, got shape {tuple(t.shape)}")
+    return t
+
+
+def _mhc_post_pre(x, residual, post_layer_mix, comb_res_mix, fn, hc_scale, hc_base, rms_eps, hc_pre_eps, hc_sinkhorn_eps,
+                  hc_post_mult_value, sinkhorn_repeat, norm_weight, norm_eps):
+    r, lead, T, H = _mhc_streams(residual)
+    fn = _mhc_f32(fn, 24 * 4 * H, "fn")
+    sc, base = _mhc_f32(hc_scale, 3, "hc_scale"), _mhc_f32(hc_base, 24, "hc_base")
+    post = x is not None
+    if post:
+        x = _cuda(x, "x")
+        if x.dtype != torch.bfloat16 or x.numel() != T * H:
+            raise ValueError(f"x must be bf16 [..., {H}] with the residual's leading shape, got {x.dtype} {tuple(x.shape)}")
+        plm = _mhc_f32(post_layer_mix, T * 4, "post_layer_mix")
+        crm = _mhc_f32(comb_res_mix, T * 16, "comb_res_mix")
+    w = None
+    if norm_weight is not None:
+        w = _cuda(norm_weight.to(torch.bfloat16), "norm_weight")
+        if w.numel() != H:
+            raise ValueError(f"norm_weight must hold {H} values, got shape {tuple(norm_weight.shape)}")
+    dev = r.device
+    r_out = torch.empty_like(r) if post else None
+    post_mix = torch.empty(*lead, 4, 1, dtype=torch.float32, device=dev)
+    comb_mix = torch.empty(*lead, 4, 4, dtype=torch.float32, device=dev)
+    layer_input = torch.empty(*lead, H, dtype=torch.bfloat16, device=dev)
+    if T:
+        ws = torch.empty(L.lib().b200_mhc_workspace_bytes(T, H), dtype=torch.uint8, device=dev)
+        rc = L.lib().b200_mhc_post_pre(
+            _stream(), x.data_ptr() if post else None, r.data_ptr(), plm.data_ptr() if post else None,
+            crm.data_ptr() if post else None, fn.data_ptr(), sc.data_ptr(), base.data_ptr(),
+            w.data_ptr() if w is not None else None, T, H, float(rms_eps), float(hc_pre_eps), float(hc_sinkhorn_eps),
+            float(hc_post_mult_value), int(sinkhorn_repeat), float(norm_eps), ws.data_ptr(),
+            r_out.data_ptr() if post else None, post_mix.data_ptr(), comb_mix.data_ptr(), layer_input.data_ptr())
+        L.check(rc, "b200_mhc_post_pre")
+    return r_out, post_mix, comb_mix, layer_input
+
+
+def mhc_pre(residual: torch.Tensor, fn: torch.Tensor, hc_scale: torch.Tensor, hc_base: torch.Tensor, rms_eps: float,
+            hc_pre_eps: float, hc_sinkhorn_eps: float, hc_post_mult_value: float, sinkhorn_repeat: int,
+            norm_weight: torch.Tensor | None = None, norm_eps: float = 1e-6):
+    """DeepSeek-V4 mHC pre mapping (the reference's mhc_pre_tilelang; kernels/mhc/torch.py:6-91 without the norm).
+    residual bf16 [..., 4, H], fn f32 [24, 4H], hc_scale f32 [3], hc_base f32 [24].  The fp32 row's RMS-scaled projection
+    gives pre gates, post gates (times hc_post_mult_value) and a 4 x 4 Sinkhorn-normalised mixing matrix; layer_input is the
+    pre-gated sum of the streams, RMS-normalised with norm_weight (cast to bf16) when given, as the reference's fused
+    kernel does (mean square of the unrounded fp32 row, applied to its bf16 rounding).
+    Returns post_mix f32 [..., 4, 1], comb_mix f32 [..., 4, 4], layer_input bf16 [..., H]."""
+    _, post_mix, comb_mix, layer_input = _mhc_post_pre(None, residual, None, None, fn, hc_scale, hc_base, rms_eps, hc_pre_eps,
+                                                       hc_sinkhorn_eps, hc_post_mult_value, sinkhorn_repeat, norm_weight,
+                                                       norm_eps)
+    return post_mix, comb_mix, layer_input
+
+
+def mhc_post(x: torch.Tensor, residual: torch.Tensor, post_layer_mix: torch.Tensor,
+             comb_res_mix: torch.Tensor) -> torch.Tensor:
+    """DeepSeek-V4 mHC post mapping (the reference's mhc_post_tilelang; torch.py:94-106): x bf16 [..., H], residual bf16
+    [..., 4, H], post_layer_mix f32 [..., 4] or [..., 4, 1], comb_res_mix f32 [..., 4, 4];
+    out[..., j, :] = bf16(post[j] x + sum_i comb[i, j] residual[i]) in fp32.  Returns bf16 [..., 4, H]."""
+    r, lead, T, H = _mhc_streams(residual)
+    x = _cuda(x, "x")
+    if x.dtype != torch.bfloat16 or x.numel() != T * H:
+        raise ValueError(f"x must be bf16 [..., {H}] with the residual's leading shape, got {x.dtype} {tuple(x.shape)}")
+    plm = _mhc_f32(post_layer_mix, T * 4, "post_layer_mix")
+    crm = _mhc_f32(comb_res_mix, T * 16, "comb_res_mix")
+    out = torch.empty_like(r)
+    if T:
+        rc = L.lib().b200_mhc_post(_stream(), x.data_ptr(), r.data_ptr(), plm.data_ptr(), crm.data_ptr(), T, H, out.data_ptr())
+        L.check(rc, "b200_mhc_post")
+    return out
+
+
+def mhc_fused_post_pre(x: torch.Tensor, residual: torch.Tensor, post_layer_mix: torch.Tensor, comb_res_mix: torch.Tensor,
+                       fn: torch.Tensor, hc_scale: torch.Tensor, hc_base: torch.Tensor, rms_eps: float, hc_pre_eps: float,
+                       hc_sinkhorn_eps: float, hc_post_mult_value: float, sinkhorn_repeat: int,
+                       norm_weight: torch.Tensor | None = None, norm_eps: float = 1e-6):
+    """mhc_post followed by the next sublayer's mhc_pre in one call (the reference's mhc_fused_post_pre_tilelang).  The mixes
+    are computed from the bf16 residual the call returns, so the result is bit-identical to
+    mhc_pre(mhc_post(x, residual, post_layer_mix, comb_res_mix), ...).
+    Returns residual_cur bf16 [..., 4, H], post_mix f32 [..., 4, 1], comb_mix f32 [..., 4, 4], layer_input bf16 [..., H]."""
+    return _mhc_post_pre(x, residual, post_layer_mix, comb_res_mix, fn, hc_scale, hc_base, rms_eps, hc_pre_eps,
+                         hc_sinkhorn_eps, hc_post_mult_value, sinkhorn_repeat, norm_weight, norm_eps)
+
+
+def hc_head(hidden_states: torch.Tensor, hc_fn: torch.Tensor, hc_scale: torch.Tensor, hc_base: torch.Tensor,
+            rms_norm_eps: float, hc_eps: float) -> torch.Tensor:
+    """DeepSeek-V4 hc_head (the reference's hc_head_fused_kernel_tilelang): collapses the 4 streams before the final norm.
+    hidden_states bf16 [T, 4, H], hc_fn f32 [4, 4H], hc_scale f32 [1], hc_base f32 [4];
+    out = bf16(sum_i (sigmoid(mix_i * rsqrt(mean(r_flat^2) + rms_norm_eps) * s + base_i) + hc_eps) r_i).  Returns bf16 [T, H]."""
+    r, lead, T, H = _mhc_streams(hidden_states, "hidden_states")
+    fn = _mhc_f32(hc_fn, 4 * 4 * H, "hc_fn")
+    sc, base = _mhc_f32(hc_scale, 1, "hc_scale"), _mhc_f32(hc_base, 4, "hc_base")
+    out = torch.empty(*lead, H, dtype=torch.bfloat16, device=r.device)
+    if T:
+        ws = torch.empty(L.lib().b200_mhc_workspace_bytes(T, H), dtype=torch.uint8, device=r.device)
+        rc = L.lib().b200_hc_head(_stream(), r.data_ptr(), fn.data_ptr(), sc.data_ptr(), base.data_ptr(), T, H,
+                                  float(rms_norm_eps), float(hc_eps), ws.data_ptr(), out.data_ptr())
+        L.check(rc, "b200_hc_head")
+    return out
+
+
 def mla_rope_cache_write(q_pe: torch.Tensor, k_pe: torch.Tensor, kv_c: torch.Tensor, positions: torch.Tensor,
                          cos_sin_cache: torch.Tensor, slot_mapping: torch.Tensor, kv_cache: torch.Tensor,
                          is_neox_style: bool = False, kv_scale: float = 1.0) -> None:
