@@ -59,7 +59,8 @@ typedef struct b200moe_config {
   int32_t group_max_len;
   int32_t groupN;           /* weight rows per scale row */
   int32_t groupK;           /* weight cols per scale col */
-  int32_t activation_type;  /* 0 silu, 1 swigluoai (layout stated by B200MOE_SWIGLUOAI_LAYOUT), 2 relu^2 (non-gated) */
+  int32_t activation_type;  /* 0 silu, 1 swigluoai (layout stated by B200MOE_SWIGLUOAI_LAYOUT), 2 relu^2 (non-gated),
+                               3 silu(min(gate, limit)) * clamp(up, -limit, limit) (DeepSeek-V4; swiglu_limit > 0) */
   float swiglu_alpha;
   float swiglu_limit;
   int32_t use_gpu_prefill;
@@ -121,12 +122,19 @@ int b200moe_gpu_prefill(b200moe_handle h, const void* hidden, void* out, const i
                         const float* topk_weights, int num_tokens, int top_k, void* stream);
 
 /* ---- routing operators ---------------------------------------------------------------------------- */
-/* softmax (scoring=0) / sigmoid (scoring=1) top-k; logits [M,E] f32/bf16/f16 (logits_dtype 0 f32, 1 bf16,
- * 2 f16); bias f32 [E] or NULL (selection only); ids int32 [M,k], weights f32 [M,k],
- * token_expert_indices int32 [M,k] = j*M+t or NULL.  Ties -> lower expert index. */
+/* softmax (scoring=0) / sigmoid (scoring=1) / sqrt(softplus) (scoring=2, DeepSeek-V4) top-k; logits [M,E] f32/bf16/f16
+ * (logits_dtype 0 f32, 1 bf16, 2 f16); bias f32 [E] or NULL (selection only: weights are the unbiased scores);
+ * ids int32 [M,k], weights f32 [M,k], token_expert_indices int32 [M,k] = j*M+t or NULL.  Ties -> lower expert index. */
 int b200_topk_gating(void* stream, const void* logits, int logits_dtype, const float* bias, int num_tokens,
                      int num_experts, int top_k, int scoring, int renormalize, float routed_scaling_factor,
                      float* topk_weights, int32_t* topk_ids, int32_t* token_expert_indices);
+/* DeepSeek-V4 hash routing (topk_softplus_sqrt_kernels.cu:326-403): ids[t] = tid2eid[input_ids[t], :] (int32 table
+ * [vocab, top_k], top_k <= 32), weights = sqrt(softplus(logits)) of those experts, renormalised (optional) and scaled
+ * by routed_scaling_factor.  No bias.  An input id outside [0, vocab) gives the whole row, a table entry outside
+ * [0, E) its slot, id -1 and weight 0. */
+int b200_hash_topk(void* stream, const void* logits, int logits_dtype, const int32_t* input_ids, const int32_t* tid2eid,
+                   int vocab, int num_tokens, int num_experts, int top_k, int renormalize, float routed_scaling_factor,
+                   float* topk_weights, int32_t* topk_ids);
 /* DeepSeek group-limited routing (scoring 0 none, 1 sigmoid); bias f32 [E] or NULL. */
 int b200_grouped_topk(void* stream, const void* logits, int logits_dtype, const float* bias, int num_tokens,
                       int num_experts, int n_group, int topk_group, int top_k, int scoring, int renormalize,
@@ -141,7 +149,7 @@ int b200_global_to_local_ids(void* stream, const int32_t* topk_ids, const int32_
  * (fused_topk_router.py:81-124, grouped_topk_kernels.cu:523-678) + global_to_local_expert_ids (routed_experts.py:1332-1342).
  * hidden [M,H] and gate_weight [E,H] in the activation dtype (16-byte aligned, H % 64 == 0, E <= 1024);
  * mode 0 softmax top-k, 1 sigmoid top-k (bias for selection only), 2 grouped top-k (scoring 0 none / 1 sigmoid, bias,
- * n_group, topk_group); topk_ids are GLOBAL expert ids; local_ids (optional) = expert_map[id] (-1 stays -1; with
+ * n_group, topk_group), 3 sqrt-softplus top-k (DeepSeek-V4, bias for selection only); topk_ids are GLOBAL expert ids; local_ids (optional) = expert_map[id] (-1 stays -1; with
  * expert_map NULL a copy); logits_out (optional) f32 [M,E].
  * Shared experts (reference runner/shared_experts.py; SURVEY.md 8f row 2) are folded into the routed launch as always-on
  * experts: with n_shared > 0 every output row has top_k + n_shared columns, the extra ones carrying weight
@@ -155,6 +163,15 @@ int b200_router_topk(void* stream, const void* hidden, int act_dtype, const void
                      int n_group, int topk_group, float routed_scaling_factor, const int32_t* expert_map, int n_shared,
                      int shared_local_base, float shared_weight, void* workspace, int64_t workspace_bytes,
                      float* topk_weights, int32_t* topk_ids, int32_t* local_ids, float* logits_out);
+/* The fused router with DeepSeek-V4 hash routing (mode must be 3): the same GEMM, then the routing of b200_hash_topk on
+ * the token's logits; EP remap, shared columns and logits_out as in b200_router_topk. */
+int b200_router_hash_topk(void* stream, const void* hidden, int act_dtype, const void* gate_weight, int num_tokens,
+                          int num_experts, int hidden_size, const float* bias, int mode, int scoring, int top_k,
+                          int renormalize, int n_group, int topk_group, float routed_scaling_factor,
+                          const int32_t* expert_map, int n_shared, int shared_local_base, float shared_weight,
+                          void* workspace, int64_t workspace_bytes, float* topk_weights, int32_t* topk_ids,
+                          int32_t* local_ids, float* logits_out, const int32_t* input_ids, const int32_t* tid2eid,
+                          int vocab);
 
 /* ---- permutation operators (stable sort by expert) ------------------------------------------------- */
 /* sorted_slot int32 [M*k] (source slot t*k+j of each permuted row, valid rows first in (expert, slot)

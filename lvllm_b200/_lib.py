@@ -50,11 +50,14 @@ PROTOTYPES = {
     "b200moe_cpu_prefill": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp]),
     "b200moe_gpu_prefill": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
     "b200_topk_gating": (_i32, [_vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp]),
+    "b200_hash_topk": (_i32, [_vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
     "b200_grouped_topk": (_i32, [_vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
     "b200_global_to_local_ids": (_i32, [_vp, _vp, _vp, _i32, _i64, _vp]),
     "b200_router_workspace_bytes": (_i64, [_i32, _i32, _i32]),
     "b200_router_topk": (_i32, [_vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _f32, _vp,
                                 _i32, _i32, _f32, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "b200_router_hash_topk": (_i32, [_vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _f32,
+                                     _vp, _i32, _i32, _f32, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),
     "b200_moe_permute": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "b200_moe_unpermute": (_i32, [_vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _vp, _i32]),
     "b200_rmsnorm_cast": (_i32, [_vp, _vp, _vp, _i32, _i32, _f32, _f32, _i32]),

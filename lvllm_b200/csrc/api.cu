@@ -267,6 +267,16 @@ int b200moe_create_empty(const b200moe_config* cfg, int format, int act_dtype, b
     set_error("b200moe_create: null config / output");
     return B200_ERR_INVALID;
   }
+  if (cfg->activation_type < 0 || cfg->activation_type > 3) {
+    set_error("b200moe_create: activation_type must be 0 silu, 1 swigluoai, 2 relu^2 or 3 silu with clamp");
+    return B200_ERR_INVALID;
+  }
+  // activation_type 3 (DeepSeek-V4): gate = min(gate, limit), up = clamp(up, -limit, limit), silu(gate) * up.  Type 3
+  // has no default limit: 0 would clamp every gate to 0.
+  if (cfg->activation_type == 3 && !(cfg->swiglu_limit > 0.f)) {
+    set_error("b200moe_create: activation_type 3 needs swiglu_limit > 0");
+    return B200_ERR_INVALID;
+  }
   int dev = 0;
   int rc = check_device(&dev);
   if (rc) return rc;

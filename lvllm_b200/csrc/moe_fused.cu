@@ -52,7 +52,7 @@ struct FusedArgs {
   int w4_tile_bytes, w4_scale_bytes;
   const float* g13;         // nvfp4 per-expert global scales [E][2] / [E]
   const float* g2;
-  float alpha, limit;
+  float alpha, limit, silu_limit;   // silu_limit: type 3's clamp, +inf for plain SiLU (type 0)
   // call
   const uint16_t* hidden;
   const int32_t* ids;
@@ -1303,7 +1303,10 @@ __global__ void __launch_bounds__((FCfg<FP8, NA, TNMAX, WQ>::NTHREADS), 1)
                     const float uu = fminf(fmaxf(u0, -a.limit), a.limit);
                     r = (uu + 1.0f) * __fdividef(gg, 1.0f + __expf(-a.alpha * gg));
                   } else {
-                    r = __fdividef(g0, 1.0f + __expf(-g0)) * u0;   // SiLU(g) * u, fast intrinsics (fp32, ~1e-6 rel)
+                    // SiLU(g) * u, fast intrinsics (fp32, ~1e-6 rel), with DeepSeek-V4's clamp for type 3.  Types 0 and 3
+                    // share the instructions: for type 0 the limit is +inf, which leaves every non-NaN value unchanged.
+                    const float gg = fminf(g0, a.silu_limit), uu = fminf(fmaxf(u0, -a.silu_limit), a.silu_limit);
+                    r = __fdividef(gg, 1.0f + __expf(-gg)) * uu;
                   }
                 } else {
                   const float t = fmaxf(g0, 0.f);
@@ -1524,6 +1527,7 @@ int launch_fused(const b200moe_layer* L, Workspace* ws, cudaStream_t st, const v
   a.g2 = L->g2;
   a.alpha = L->cfg.swiglu_alpha;
   a.limit = L->cfg.swiglu_limit;
+  a.silu_limit = L->cfg.activation_type == 3 ? L->cfg.swiglu_limit : INFINITY;
   a.hidden = reinterpret_cast<const uint16_t*>(hidden);
   a.ids = ids;
   a.topk_w = topk_w;

@@ -58,8 +58,8 @@ struct GemmArgs {
   int KB_out;           // k-blocks of the NEXT GEMM's operand (intermediate width / elems-per-128B)
   int rows_stride;      // stride of the transposed scale arrays
   int n_out;            // leading dim of y
-  int act_type;         // 0 silu, 1 swigluoai, 2 relu2
-  float alpha, limit;
+  int act_type;         // 0 silu, 1 swigluoai, 2 relu2, 3 silu with clamp
+  float alpha, limit, silu_limit;   // silu_limit: type 3's clamp, +inf for plain SiLU (type 0)
   int act_fp16;         // activation dtype of the 16-bit intermediate: 0 bf16, 1 fp16
   int e8m0;             // FP8 layers in ue8m0 mode: activation / intermediate group scales are rounded up to powers of two
 };
@@ -363,7 +363,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) moe_gemm_kernel(const GemmArg
               const float uu = fminf(fmaxf(u0, -a.limit), a.limit);
               r = (uu + 1.0f) * gg * (1.0f / (1.0f + expf(-a.alpha * gg)));
             } else {
-              r = silu_f(g0) * u0;
+              // SiLU, with DeepSeek-V4's clamp for type 3; for type 0 the limit is +inf (every non-NaN value unchanged)
+              r = silu_f(fminf(g0, a.silu_limit)) * fminf(fmaxf(u0, -a.silu_limit), a.silu_limit);
             }
           } else {
             const float t = fmaxf(g0, 0.f);
@@ -459,6 +460,7 @@ static int launch_pair(const b200moe_layer* L, Workspace* ws, cudaStream_t st, i
   g1.act_type = L->cfg.activation_type;
   g1.alpha = L->cfg.swiglu_alpha;
   g1.limit = L->cfg.swiglu_limit;
+  g1.silu_limit = L->cfg.activation_type == 3 ? L->cfg.swiglu_limit : INFINITY;
   g1.act_fp16 = (L->act_dtype == B200_ACT_FP16);
   g1.e8m0 = L->fp8_e8m0;
   int rc;

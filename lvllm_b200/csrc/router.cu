@@ -36,12 +36,14 @@ struct RouterArgs {
   float* partial;        // [KS][M][Epad]
   int32_t* counters;     // [token tiles], zero between launches
   float* logits_out;     // optional [M][E]
-  int mode;              // 0 softmax top-k, 1 sigmoid top-k, 2 grouped top-k
+  int mode;              // 0 softmax top-k, 1 sigmoid top-k, 2 grouped top-k, 3 sqrt-softplus top-k (or hash)
   int scoring;           // grouped: 0 none, 1 sigmoid
   int k, renorm, n_group, topk_group;
   float rsf;
   const float* bias;
   const int32_t* emap;   // optional global -> local expert ids
+  const int32_t* input_ids, *tid2eid;   // hash routing (mode 3): ids = tid2eid[input_ids[t]], tid2eid [vocab][k]
+  int vocab;
   // shared experts folded into the routed launch as always-on experts (SURVEY.md 8f row 2): n_shared extra columns per
   // token, weight shared_w; global id E + s, local id shared_local_base + s (or -1 when this rank does not hold them)
   int n_shared, shared_local_base;
@@ -234,8 +236,11 @@ __global__ void __launch_bounds__(R_THREADS, 1) router_gemm_topk_kernel(const __
       float* sc = scratch + (size_t)warp * 2 * a.Epad;
       route_row_grouped(row, sc, sc + a.Epad, a.bias, a.E, a.n_group, a.topk_group, a.k, a.scoring, a.renorm, a.rsf, a.out_w,
                         a.out_ids, tg, lane, ld);
+    } else if (a.tid2eid) {
+      route_row_hash(row, a.input_ids[tg], a.tid2eid, a.vocab, a.E, a.k, a.renorm, a.rsf, a.out_w, a.out_ids, tg, lane, ld);
     } else {
-      route_row_topk(row, a.bias, a.E, a.k, a.mode, a.renorm, a.rsf, a.out_w, a.out_ids, nullptr, tg, a.M, lane, ld);
+      route_row_topk(row, a.bias, a.E, a.k, a.mode == 3 ? 2 : a.mode, a.renorm, a.rsf, a.out_w, a.out_ids, nullptr, tg,
+                     a.M, lane, ld);
     }
     __syncwarp();
     for (int j = lane; j < a.n_shared; j += 32) {
@@ -298,32 +303,43 @@ int64_t b200_router_workspace_bytes(int num_tokens, int num_experts, int hidden_
   return counters + (int64_t)KS * num_tokens * EZ * 128 * 4;
 }
 
-int b200_router_topk(void* stream, const void* hidden, int act_dtype, const void* gate_weight, int num_tokens,
-                     int num_experts, int hidden_size, const float* bias, int mode, int scoring, int top_k, int renormalize,
-                     int n_group, int topk_group, float routed_scaling_factor, const int32_t* expert_map, int n_shared,
-                     int shared_local_base, float shared_weight, void* workspace, int64_t workspace_bytes,
-                     float* topk_weights, int32_t* topk_ids, int32_t* local_ids, float* logits_out) {
+}  // extern "C"
+
+// b200_router_topk and b200_router_hash_topk: tid2eid NULL routes by top-k
+static int router_launch(const char* name, void* stream, const void* hidden, int act_dtype, const void* gate_weight,
+                         int num_tokens, int num_experts, int hidden_size, const float* bias, int mode, int scoring,
+                         int top_k, int renormalize, int n_group, int topk_group, float routed_scaling_factor,
+                         const int32_t* expert_map, int n_shared, int shared_local_base, float shared_weight,
+                         void* workspace, int64_t workspace_bytes, float* topk_weights, int32_t* topk_ids,
+                         int32_t* local_ids, float* logits_out, const int32_t* input_ids, const int32_t* tid2eid,
+                         int vocab) {
+  const std::string fn(name);
+
   const int M = num_tokens, E = num_experts, H = hidden_size;
   if (!hidden || !gate_weight || !workspace || !topk_weights || !topk_ids || E <= 0 || E > MAX_EXPERTS || H <= 0 || H % 64 ||
-      top_k <= 0 || top_k > E || mode < 0 || mode > 2 || n_shared < 0 || n_shared > 8 ||
+      top_k <= 0 || top_k > E || mode < 0 || mode > 3 || n_shared < 0 || n_shared > 8 ||
       (act_dtype != B200_ACT_BF16 && act_dtype != B200_ACT_FP16)) {
-    set_error("b200_router_topk: bad argument (E <= 1024, H % 64 == 0, mode 0|1|2)");
+    set_error(fn + ": bad argument (E <= 1024, H % 64 == 0, mode 0|1|2|3)");
     return B200_ERR_INVALID;
   }
   if (mode == 2 && (n_group <= 0 || n_group > 32 || E % n_group || topk_group <= 0 || topk_group > n_group ||
                     (scoring != 0 && scoring != 1))) {
-    set_error("b200_router_topk: bad grouped-routing argument (n_group <= 32, E % n_group == 0)");
+    set_error(fn + ": bad grouped-routing argument (n_group <= 32, E % n_group == 0)");
+    return B200_ERR_INVALID;
+  }
+  if (tid2eid && (!input_ids || vocab <= 0 || mode != 3 || top_k > 32)) {
+    set_error(fn + ": bad hash-routing argument (input_ids non-NULL, vocab > 0, mode 3, top_k <= 32)");
     return B200_ERR_INVALID;
   }
   if (M <= 0) return 0;
   if (((uintptr_t)hidden & 15) || ((uintptr_t)gate_weight & 15)) {
-    set_error("b200_router_topk: hidden / gate_weight must be 16-byte aligned");
+    set_error(fn + ": hidden / gate_weight must be 16-byte aligned");
     return B200_ERR_INVALID;
   }
   int TN, TT, EZ, KS;
   router_shape(M, E, H, &TN, &TT, &EZ, &KS);
   if (workspace_bytes < b200_router_workspace_bytes(M, E, H)) {
-    set_error("b200_router_topk: workspace too small (b200_router_workspace_bytes)");
+    set_error(fn + ": workspace too small (b200_router_workspace_bytes)");
     return B200_ERR_INVALID;
   }
   RouterArgs a{};
@@ -366,6 +382,9 @@ int b200_router_topk(void* stream, const void* hidden, int act_dtype, const void
   a.rsf = routed_scaling_factor;
   a.bias = bias;
   a.emap = expert_map;
+  a.input_ids = input_ids;
+  a.tid2eid = tid2eid;
+  a.vocab = vocab;
   a.out_w = topk_weights;
   a.out_ids = topk_ids;
   a.out_local = local_ids;
@@ -381,6 +400,36 @@ int b200_router_topk(void* stream, const void* hidden, int act_dtype, const void
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "router launch");
   return 0;
+}
+
+extern "C" {
+
+int b200_router_topk(void* stream, const void* hidden, int act_dtype, const void* gate_weight, int num_tokens,
+                     int num_experts, int hidden_size, const float* bias, int mode, int scoring, int top_k, int renormalize,
+                     int n_group, int topk_group, float routed_scaling_factor, const int32_t* expert_map, int n_shared,
+                     int shared_local_base, float shared_weight, void* workspace, int64_t workspace_bytes,
+                     float* topk_weights, int32_t* topk_ids, int32_t* local_ids, float* logits_out) {
+  return router_launch("b200_router_topk", stream, hidden, act_dtype, gate_weight, num_tokens, num_experts, hidden_size,
+                       bias, mode, scoring, top_k, renormalize, n_group, topk_group, routed_scaling_factor, expert_map,
+                       n_shared, shared_local_base, shared_weight, workspace, workspace_bytes, topk_weights, topk_ids,
+                       local_ids, logits_out, nullptr, nullptr, 0);
+}
+
+int b200_router_hash_topk(void* stream, const void* hidden, int act_dtype, const void* gate_weight, int num_tokens,
+                          int num_experts, int hidden_size, const float* bias, int mode, int scoring, int top_k,
+                          int renormalize, int n_group, int topk_group, float routed_scaling_factor,
+                          const int32_t* expert_map, int n_shared, int shared_local_base, float shared_weight,
+                          void* workspace, int64_t workspace_bytes, float* topk_weights, int32_t* topk_ids,
+                          int32_t* local_ids, float* logits_out, const int32_t* input_ids, const int32_t* tid2eid,
+                          int vocab) {
+  if (!tid2eid) {
+    set_error("b200_router_hash_topk: tid2eid is NULL");
+    return B200_ERR_INVALID;
+  }
+  return router_launch("b200_router_hash_topk", stream, hidden, act_dtype, gate_weight, num_tokens, num_experts,
+                       hidden_size, bias, mode, scoring, top_k, renormalize, n_group, topk_group, routed_scaling_factor,
+                       expert_map, n_shared, shared_local_base, shared_weight, workspace, workspace_bytes, topk_weights,
+                       topk_ids, local_ids, logits_out, input_ids, tid2eid, vocab);
 }
 
 }  // extern "C"

@@ -1,5 +1,7 @@
 // Routing + permutation operators (latency / HBM bound integer & fp32 work; one warp per token).
-//   b200_topk_gating      softmax / sigmoid top-k, lower-index tie-break     (reference topk_softmax_kernels.cu:408-592)
+//   b200_topk_gating      softmax / sigmoid / sqrt-softplus top-k, lower-index tie-break
+//                                                                             (reference topk_softmax_kernels.cu:408-592)
+//   b200_hash_topk        DeepSeek-V4 token-id hash routing                  (reference topk_softplus_sqrt_kernels.cu:326-403)
 //   b200_grouped_topk     DeepSeek group-limited routing                     (reference grouped_topk_kernels.cu:477-675)
 //   b200_global_to_local_ids                                                  (reference routed_experts.py:1332-1342)
 //   b200_moe_permute / b200_moe_unpermute   stable sort by expert, gather, fp32 weighted reduce
@@ -15,7 +17,8 @@ constexpr int MAX_VPT = MAX_EXPERTS / 32;
 __global__ void __launch_bounds__(ROUTE_WARPS * 32)
     topk_gating_kernel(const void* __restrict__ logits, int dtype, const float* __restrict__ bias, int M, int E, int k,
                        int scoring, int renorm, float rsf, float* __restrict__ out_w, int32_t* __restrict__ out_ids,
-                       int32_t* __restrict__ tok_exp_idx) {
+                       int32_t* __restrict__ tok_exp_idx, const int32_t* __restrict__ input_ids,
+                       const int32_t* __restrict__ tid2eid, int vocab) {
   extern __shared__ float sm[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t = blockIdx.x * ROUTE_WARPS + warp;
@@ -23,7 +26,10 @@ __global__ void __launch_bounds__(ROUTE_WARPS * 32)
   float* p = sm + (size_t)warp * E;
   for (int e = lane; e < E; e += 32) p[e] = load_logit(logits, dtype, (size_t)t * E + e);
   __syncwarp();
-  route_row_topk(p, bias, E, k, scoring, renorm, rsf, out_w, out_ids, tok_exp_idx, t, M, lane, k);
+  if (tid2eid)
+    route_row_hash(p, input_ids[t], tid2eid, vocab, E, k, renorm, rsf, out_w, out_ids, t, lane, k);
+  else
+    route_row_topk(p, bias, E, k, scoring, renorm, rsf, out_w, out_ids, tok_exp_idx, t, M, lane, k);
 }
 
 __global__ void __launch_bounds__(ROUTE_WARPS * 32)
@@ -212,8 +218,8 @@ int b200_topk_gating(void* stream, const void* logits, int logits_dtype, const f
                      int num_experts, int top_k, int scoring, int renormalize, float routed_scaling_factor,
                      float* topk_weights, int32_t* topk_ids, int32_t* token_expert_indices) {
   if (!logits || !topk_weights || !topk_ids || num_experts <= 0 || num_experts > MAX_EXPERTS || top_k <= 0 ||
-      top_k > num_experts || logits_dtype < 0 || logits_dtype > 2 || (scoring != 0 && scoring != 1)) {
-    set_error("b200_topk_gating: bad argument");
+      top_k > num_experts || logits_dtype < 0 || logits_dtype > 2 || scoring < 0 || scoring > 2) {
+    set_error("b200_topk_gating: bad argument (scoring 0 softmax | 1 sigmoid | 2 sqrtsoftplus)");
     return B200_ERR_INVALID;
   }
   if (num_tokens <= 0) return 0;
@@ -221,10 +227,31 @@ int b200_topk_gating(void* stream, const void* logits, int logits_dtype, const f
   const size_t smem = (size_t)ROUTE_WARPS * num_experts * sizeof(float);
   topk_gating_kernel<<<grid, ROUTE_WARPS * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
       logits, logits_dtype, bias, num_tokens, num_experts, top_k, scoring, renormalize, routed_scaling_factor,
-      topk_weights, topk_ids, token_expert_indices);
+      topk_weights, topk_ids, token_expert_indices, nullptr, nullptr, 0);
   ++g_launches;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "topk_gating launch");
+  return 0;
+}
+
+int b200_hash_topk(void* stream, const void* logits, int logits_dtype, const int32_t* input_ids, const int32_t* tid2eid,
+                   int vocab, int num_tokens, int num_experts, int top_k, int renormalize, float routed_scaling_factor,
+                   float* topk_weights, int32_t* topk_ids) {
+  if (!logits || !input_ids || !tid2eid || !topk_weights || !topk_ids || vocab <= 0 || num_experts <= 0 ||
+      num_experts > MAX_EXPERTS || top_k <= 0 || top_k > 32 || top_k > num_experts || logits_dtype < 0 ||
+      logits_dtype > 2) {
+    set_error("b200_hash_topk: bad argument (table and ids non-NULL, vocab > 0, top_k <= 32)");
+    return B200_ERR_INVALID;
+  }
+  if (num_tokens <= 0) return 0;
+  const int grid = (num_tokens + ROUTE_WARPS - 1) / ROUTE_WARPS;
+  const size_t smem = (size_t)ROUTE_WARPS * num_experts * sizeof(float);
+  topk_gating_kernel<<<grid, ROUTE_WARPS * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      logits, logits_dtype, nullptr, num_tokens, num_experts, top_k, 2, renormalize, routed_scaling_factor,
+      topk_weights, topk_ids, nullptr, input_ids, tid2eid, vocab);
+  ++g_launches;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "hash_topk launch");
   return 0;
 }
 

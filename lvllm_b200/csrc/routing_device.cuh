@@ -1,6 +1,8 @@
 // Per-token routing arithmetic shared by the stand-alone routing kernels (routing.cu) and the fused router
 // (router.cu): one warp per token, scores in shared memory, k rounds of warp arg-max (ties -> lower expert index).
-//   route_row_topk     softmax / sigmoid top-k                     (reference topk_softmax_kernels.cu:408-592)
+//   route_row_topk     softmax / sigmoid / sqrt-softplus top-k     (reference topk_softmax_kernels.cu:408-592,
+//                                                                   topk_softplus_sqrt_kernels.cu:404-537)
+//   route_row_hash     DeepSeek-V4 token-id hash routing           (reference topk_softplus_sqrt_kernels.cu:326-403)
 //   route_row_grouped  DeepSeek group-limited routing              (reference grouped_topk_kernels.cu:477-675)
 #pragma once
 #include <math_constants.h>
@@ -28,8 +30,14 @@ B200_DEVICE void warp_argmax(float& v, int& idx) {
   }
 }
 
-// p[E] (shared memory): the token's raw fp32 logits on entry, overwritten by the scores.  Writes row t (row stride ld
-// >= k) of out_w / out_ids (/ tok_exp_idx).  Executed by one full warp.
+// DeepSeek-V4 score sqrt(softplus(x)), with F.softplus's threshold of 20.  Accurate expf / log1pf (not the fast
+// intrinsics) so that a float32 host oracle agrees to a few ulp.
+B200_DEVICE float sqrt_softplus(float x) { return sqrtf(x > 20.f ? x : log1pf(expf(x))); }
+
+// p[E] (shared memory): the token's raw fp32 logits on entry, overwritten by the scores (scoring 0 softmax,
+// 1 sigmoid, 2 sqrt-softplus).  Writes row t (row stride ld >= k) of out_w / out_ids (/ tok_exp_idx).  Executed by one
+// full warp.  Selection is by score + bias; the weight is the unbiased score.  For sqrt-softplus this follows the
+// reference's dsv4_topk and torch paths, not its CUDA kernel, which weights by (s + b) - b.
 B200_DEVICE void route_row_topk(float* p, const float* __restrict__ bias, int E, int k, int scoring, int renorm, float rsf,
                                 float* __restrict__ out_w, int32_t* __restrict__ out_ids, int32_t* __restrict__ tok_exp_idx,
                                 int t, int M, int lane, int ld) {
@@ -46,8 +54,10 @@ B200_DEVICE void route_row_topk(float* p, const float* __restrict__ bias, int E,
     s = warp_sum(s);
     const float r = 1.f / s;
     for (int e = lane; e < E; e += 32) p[e] *= r;
-  } else {
+  } else if (scoring == 1) {
     for (int e = lane; e < E; e += 32) p[e] = 1.0f / (1.0f + expf(-p[e]));
+  } else {
+    for (int e = lane; e < E; e += 32) p[e] = sqrt_softplus(p[e]);
   }
   for (int e = lane; e < E; e += 32) {
     const float v = p[e];
@@ -81,6 +91,32 @@ B200_DEVICE void route_row_topk(float* p, const float* __restrict__ bias, int E,
     float scale = rsf;
     if (renorm) scale = scale / (sel_sum > 0.f ? sel_sum : 1.f);
     for (int j = 0; j < k; ++j) out_w[(size_t)t * ld + j] *= scale;
+  }
+}
+
+// Hash routing of DeepSeek-V4's first layers: the experts of token t are tid2eid[token_id, 0..k) in table order (k <= 32,
+// one lane per slot), weighted by their sqrt-softplus scores; no bias.  A token id outside [0, vocab) empties the row, a
+// table entry outside [0, E) its slot: id -1, weight 0.  p[E]: the token's raw fp32 logits (read only).  One full warp.
+B200_DEVICE void route_row_hash(const float* p, int token_id, const int32_t* __restrict__ tid2eid, int vocab, int E,
+                                int k, int renorm, float rsf, float* __restrict__ out_w, int32_t* __restrict__ out_ids,
+                                int t, int lane, int ld) {
+  int id = -1;
+  float w = 0.f;
+  if (lane < k && token_id >= 0 && token_id < vocab) {
+    const int e = tid2eid[(size_t)token_id * k + lane];
+    if (e >= 0 && e < E) {
+      const float s = sqrt_softplus(p[e]);
+      id = e;
+      w = (isnan(s) || isinf(s)) ? 0.f : s;
+    }
+  }
+  float sum = 0.f;  // in slot order, like the top-k path
+  for (int j = 0; j < k; ++j) sum += __shfl_sync(0xffffffffu, w, j);
+  float scale = rsf;
+  if (renorm) scale = scale / (sum > 0.f ? sum : 1.f);
+  if (lane < k) {
+    out_ids[(size_t)t * ld + lane] = id;
+    out_w[(size_t)t * ld + lane] = w * scale;
   }
 }
 

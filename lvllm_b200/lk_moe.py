@@ -15,7 +15,12 @@ from . import _lib as L
 
 
 class MOEConfigV2:
-    """Plain attribute bag; field list of reference routed_experts.py:1490-1511."""
+    """Plain attribute bag; field list of reference routed_experts.py:1490-1511.
+
+    The reference assigns ``swiglu_limit`` explicitly only for models whose SiLU experts clamp (DeepSeek-V4,
+    routed_experts.py:1506-1510), while every config carries the default 7.0.  So the bag records whether the caller
+    assigned the limit, and ``activation_type 0`` with an assigned limit is sent to the library as type 3 (SiLU with
+    the clamp).  Other types are sent as they are."""
 
     def __init__(self):
         self.num_processes = 1
@@ -37,12 +42,20 @@ class MOEConfigV2:
         self.swiglu_alpha = 1.702
         self.swiglu_limit = 7.0
         self.use_gpu_prefill = False
+        self.swiglu_limit_assigned = False
+
+    def __setattr__(self, name, value):
+        if name == "swiglu_limit" and "swiglu_limit" in self.__dict__:
+            object.__setattr__(self, "swiglu_limit_assigned", True)
+        object.__setattr__(self, name, value)
 
     def _to_c(self) -> L.B200Config:
         c = L.B200Config()
         for name, _ in L.B200Config._fields_:
             v = getattr(self, name)
             setattr(c, name, float(v) if name.startswith("swiglu") else int(v))
+        if c.activation_type == 0 and self.swiglu_limit_assigned:
+            c.activation_type = 3
         return c
 
 

@@ -24,10 +24,21 @@ def _cuda(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
+_SCORING = {"softmax": 0, "sigmoid": 1, "sqrtsoftplus": 2}
+
+
+def _i32(t: torch.Tensor, name: str) -> torch.Tensor:
+    """int32 contiguous CUDA view; converts only when the caller passed another dtype."""
+    t = _cuda(t, name)
+    return t if t.dtype == torch.int32 else t.to(torch.int32)
+
+
 def fused_topk(gating_output: torch.Tensor, topk: int, renormalize: bool, scoring_func: str = "softmax",
                e_score_correction_bias: torch.Tensor | None = None, routed_scaling_factor: float = 1.0,
                return_token_expert_indices: bool = False):
-    """reference fused_topk_router.py:81-124 -> _moe_C.topk_softmax / topk_sigmoid."""
+    """reference fused_topk_router.py:81-124 -> _moe_C.topk_softmax / topk_sigmoid, and fused_topk_bias_router.py ->
+    topk_softplus_sqrt for ``scoring_func="sqrtsoftplus"`` (DeepSeek-V4: the bias selects, the weights are the
+    unbiased scores)."""
     g = _cuda(gating_output, "gating_output")
     M, E = g.shape
     w = torch.empty(M, topk, dtype=torch.float32, device=g.device)
@@ -35,7 +46,7 @@ def fused_topk(gating_output: torch.Tensor, topk: int, renormalize: bool, scorin
     tei = torch.empty(M, topk, dtype=torch.int32, device=g.device) if return_token_expert_indices else None
     bias = _cuda(e_score_correction_bias.float(), "bias") if e_score_correction_bias is not None else None
     rc = L.lib().b200_topk_gating(_stream(), g.data_ptr(), _DT[g.dtype], bias.data_ptr() if bias is not None else None,
-                                  M, E, topk, {"softmax": 0, "sigmoid": 1}[scoring_func], int(renormalize),
+                                  M, E, topk, _SCORING[scoring_func], int(renormalize),
                                   float(routed_scaling_factor), w.data_ptr(), ids.data_ptr(),
                                   tei.data_ptr() if tei is not None else None)
     L.check(rc, "b200_topk_gating")
@@ -63,6 +74,27 @@ def grouped_topk(gating_output: torch.Tensor, topk: int, renormalize: bool, num_
     return w, ids
 
 
+def hash_topk(gating_output: torch.Tensor, topk: int, renormalize: bool, input_ids: torch.Tensor,
+              hash_indices_table: torch.Tensor, routed_scaling_factor: float = 1.0):
+    """DeepSeek-V4 hash routing (reference topk_softplus_sqrt with ``hash_indices_table``): ids = table[input_ids], in
+    table order; weights = sqrt(softplus(logits)) of those experts.  table [vocab, topk]; ids or table entries out of
+    range give id -1 and weight 0.  Returns (topk_weights f32 [M,k], topk_ids i32 [M,k])."""
+    g = _cuda(gating_output, "gating_output")
+    M, E = g.shape
+    tab = _i32(hash_indices_table, "hash_indices_table")
+    if tab.dim() != 2 or tab.shape[1] != topk:
+        raise ValueError(f"hash_indices_table must be [vocab, {topk}], got {tuple(tab.shape)}")
+    ids_in = _i32(input_ids, "input_ids").reshape(-1)
+    if ids_in.numel() != M:
+        raise ValueError(f"input_ids has {ids_in.numel()} tokens, gating_output {M}")
+    w = torch.empty(M, topk, dtype=torch.float32, device=g.device)
+    ids = torch.empty(M, topk, dtype=torch.int32, device=g.device)
+    rc = L.lib().b200_hash_topk(_stream(), g.data_ptr(), _DT[g.dtype], ids_in.data_ptr(), tab.data_ptr(), tab.shape[0], M,
+                                E, topk, int(renormalize), float(routed_scaling_factor), w.data_ptr(), ids.data_ptr())
+    L.check(rc, "b200_hash_topk")
+    return w, ids
+
+
 _router_ws: dict = {}
 
 
@@ -70,12 +102,15 @@ def router_topk(hidden_states: torch.Tensor, gate_weight: torch.Tensor, topk: in
                 scoring_func: str = "softmax", e_score_correction_bias: torch.Tensor | None = None,
                 routed_scaling_factor: float = 1.0, num_expert_group: int = 0, topk_group: int = 0,
                 expert_map: torch.Tensor | None = None, return_logits: bool = False, n_shared: int = 0,
-                shared_local_base: int = -1, shared_weight: float = 1.0):
+                shared_local_base: int = -1, shared_weight: float = 1.0, input_ids: torch.Tensor | None = None,
+                hash_indices_table: torch.Tensor | None = None):
     """Fused router: GateLinear.forward (reference router/gate_linear.py:171-221) + fused_topk / grouped_topk
     (fused_topk_router.py:81-124, grouped_topk_router.py:28-166) + global_to_local_expert_ids in ONE kernel.
     hidden [M,H], gate_weight [E,H] (same 16-bit dtype).  ``num_expert_group > 0`` selects DeepSeek grouped routing.
     ``n_shared`` > 0 appends always-on columns for shared experts held at local ids shared_local_base + s (weight
     ``shared_weight``; reference runner/shared_experts.py) — local_ids are then always returned.
+    ``scoring_func="sqrtsoftplus"`` is DeepSeek-V4's top-k; with ``hash_indices_table`` [vocab, k] and ``input_ids``
+    it is V4's hash routing (as ``hash_topk``, on the same kernel's logits).
     Returns (topk_weights f32 [M,k'], topk_ids i32 [M,k'] global, local_ids i32 [M,k'] | None[, logits f32 [M,E]]),
     k' = k + n_shared."""
     h, wg = _cuda(hidden_states, "hidden_states"), _cuda(gate_weight, "gate_weight")
@@ -101,15 +136,27 @@ def router_topk(hidden_states: torch.Tensor, gate_weight: torch.Tensor, topk: in
         assert scoring_func in ("sigmoid", "none")
         mode, scoring = 2, 1 if scoring_func == "sigmoid" else 0
     else:
-        mode, scoring = {"softmax": 0, "sigmoid": 1}[scoring_func], 0
-    rc = lib.b200_router_topk(_stream(), h.data_ptr(), 1 if h.dtype == torch.float16 else 0, wg.data_ptr(), M, E, H,
-                              bias.data_ptr() if bias is not None else None, mode, scoring, topk, int(renormalize),
-                              int(num_expert_group), int(topk_group), float(routed_scaling_factor),
-                              em.data_ptr() if em is not None else None, int(n_shared), int(shared_local_base),
-                              float(shared_weight), ws.data_ptr(), ws.numel(), w.data_ptr(),
-                              ids.data_ptr(), loc.data_ptr() if loc is not None else None,
-                              lg.data_ptr() if lg is not None else None)
-    L.check(rc, "b200_router_topk")
+        mode, scoring = {"softmax": 0, "sigmoid": 1, "sqrtsoftplus": 3}[scoring_func], 0
+    args = (_stream(), h.data_ptr(), 1 if h.dtype == torch.float16 else 0, wg.data_ptr(), M, E, H,
+            bias.data_ptr() if bias is not None else None, mode, scoring, topk, int(renormalize),
+            int(num_expert_group), int(topk_group), float(routed_scaling_factor),
+            em.data_ptr() if em is not None else None, int(n_shared), int(shared_local_base),
+            float(shared_weight), ws.data_ptr(), ws.numel(), w.data_ptr(),
+            ids.data_ptr(), loc.data_ptr() if loc is not None else None,
+            lg.data_ptr() if lg is not None else None)
+    if hash_indices_table is None:
+        L.check(lib.b200_router_topk(*args), "b200_router_topk")
+    else:
+        if input_ids is None:
+            raise ValueError("hash routing needs input_ids")
+        tab = _i32(hash_indices_table, "hash_indices_table")
+        if tab.dim() != 2 or tab.shape[1] != topk:
+            raise ValueError(f"hash_indices_table must be [vocab, {topk}], got {tuple(tab.shape)}")
+        ids_in = _i32(input_ids, "input_ids").reshape(-1)
+        if ids_in.numel() != M:
+            raise ValueError(f"input_ids has {ids_in.numel()} tokens, hidden_states {M}")
+        L.check(lib.b200_router_hash_topk(*args, ids_in.data_ptr(), tab.data_ptr(), tab.shape[0]),
+                "b200_router_hash_topk")
     return (w, ids, loc, lg) if return_logits else (w, ids, loc)
 
 

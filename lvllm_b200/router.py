@@ -8,6 +8,8 @@ Two ways in, one way out:
     group-limited routing, grouped_topk_router.py:249-330);
   * `select_experts(hidden_states, gate_weight=W_g)` — the fused form: router GEMM + top-k + EP id remap (+ always-on shared
     expert columns) in ONE kernel (`ops.router_topk`), no logits tensor.
+DeepSeek-V4 layers use `scoring_func="sqrtsoftplus"` (the bias selects, the weights are the unbiased scores); its first
+`num_hash_layers` layers route by `hash_indices_table` [vocab, k] instead, reading `input_ids` in `select_experts`.
 Both return `(topk_weights f32 [M, k'], topk_ids [M, k'])` with GLOBAL logical ids, like the reference; the EP-local ids lk_moe
 consumes (`RoutedExperts.global_to_local_expert_ids`, routed_experts.py:1332-1342) are kept in `last_local_ids`.
 Host-side glue only: every tensor operation is one of the C-ABI kernels behind `lvllm_b200.ops`.
@@ -26,15 +28,23 @@ class Router:
                  num_expert_group: int = 0, topk_group: int = 0, routed_scaling_factor: float = 1.0,
                  e_score_correction_bias: torch.Tensor | None = None, expert_map: torch.Tensor | None = None,
                  num_fused_shared_experts: int = 0, shared_local_base: int = -1, shared_weight: float = 1.0,
-                 capture_fn: Callable[[torch.Tensor], None] | None = None, eplb_state=None):
+                 capture_fn: Callable[[torch.Tensor], None] | None = None, eplb_state=None,
+                 hash_indices_table: torch.Tensor | None = None):
         if top_k <= 0 or global_num_experts <= 0 or top_k > global_num_experts:
             raise ValueError(f"bad top_k / global_num_experts: {top_k} / {global_num_experts}")
         if (num_expert_group > 0) != (topk_group > 0):
             raise ValueError("num_expert_group and topk_group are set together (grouped routing) or not at all")
         if num_expert_group > 0 and (global_num_experts % num_expert_group or topk_group > num_expert_group):
             raise ValueError("grouped routing: experts must divide into the groups and topk_group <= num_expert_group")
-        if scoring_func not in ("softmax", "sigmoid"):
+        if scoring_func not in ("softmax", "sigmoid", "sqrtsoftplus"):
             raise ValueError(f"unsupported scoring function {scoring_func!r}")
+        if scoring_func == "sqrtsoftplus" and num_expert_group > 0:
+            raise ValueError("grouped routing with sqrtsoftplus scores is not supported")
+        if hash_indices_table is not None:
+            if scoring_func != "sqrtsoftplus":
+                raise ValueError("hash routing weights experts by sqrtsoftplus scores: pass scoring_func='sqrtsoftplus'")
+            if hash_indices_table.dim() != 2 or hash_indices_table.shape[1] != top_k:
+                raise ValueError(f"hash_indices_table must be [vocab, {top_k}], got {tuple(hash_indices_table.shape)}")
         if eplb_state is not None:
             # EPLB (redundant physical experts, vllm/distributed/eplb) is outside the hot-path scope (SURVEY.md 2): refusing
             # is better than silently routing to logical ids
@@ -50,11 +60,16 @@ class Router:
         self.num_fused_shared_experts = int(num_fused_shared_experts)
         self.shared_local_base, self.shared_weight = int(shared_local_base), float(shared_weight)
         self.capture_fn = capture_fn
+        # int32 once here, so that the per-step call converts nothing
+        self.hash_indices_table = hash_indices_table.to(torch.int32).contiguous() if hash_indices_table is not None else None
         self.last_local_ids: torch.Tensor | None = None
 
     # ---- step 2 of the template: the routing algorithm -----------------------------------------------------------
     def _compute_routing(self, hidden_states: torch.Tensor, router_logits: torch.Tensor | None,
-                         gate_weight: torch.Tensor | None):
+                         gate_weight: torch.Tensor | None, input_ids: torch.Tensor | None):
+        hashed = self.hash_indices_table is not None
+        if hashed and input_ids is None:
+            raise ValueError("this router's layer routes by token-id hash: select_experts needs input_ids")
         if gate_weight is not None:
             if gate_weight.shape[0] != self.global_num_experts:
                 raise ValueError(f"gate_weight has {gate_weight.shape[0]} rows, the router {self.global_num_experts} experts")
@@ -64,7 +79,9 @@ class Router:
             w, ids, loc = ops.router_topk(hidden_states, gate_weight, self.top_k, self.renormalize, self.scoring_func,
                                           self.e_score_correction_bias, self.routed_scaling_factor, self.num_expert_group,
                                           self.topk_group, self.expert_map, False, self.num_fused_shared_experts,
-                                          self.shared_local_base, self.shared_weight)
+                                          self.shared_local_base, self.shared_weight,
+                                          **(dict(input_ids=input_ids, hash_indices_table=self.hash_indices_table)
+                                             if hashed else {}))
             return w, ids, loc
         if router_logits is None:
             raise ValueError("select_experts needs router_logits or gate_weight")
@@ -75,6 +92,9 @@ class Router:
         if self.num_expert_group > 0:
             w, ids = ops.grouped_topk(router_logits, self.top_k, self.renormalize, self.num_expert_group, self.topk_group,
                                       self.scoring_func, self.routed_scaling_factor, self.e_score_correction_bias)
+        elif hashed:
+            w, ids = ops.hash_topk(router_logits, self.top_k, self.renormalize, input_ids, self.hash_indices_table,
+                                   self.routed_scaling_factor)
         else:
             w, ids = ops.fused_topk(router_logits, self.top_k, self.renormalize, self.scoring_func,
                                     self.e_score_correction_bias, self.routed_scaling_factor)
@@ -85,8 +105,9 @@ class Router:
     def select_experts(self, hidden_states: torch.Tensor, router_logits: torch.Tensor | None = None,
                        topk_indices_dtype: torch.dtype | None = None, *, input_ids: torch.Tensor | None = None,
                        gate_weight: torch.Tensor | None = None):
-        """`input_ids` is part of the reference's signature (hash-routed models); the routing methods here do not read it."""
-        topk_weights, topk_ids, local_ids = self._compute_routing(hidden_states, router_logits, gate_weight)
+        """`input_ids` [M] are the token ids; read only by a hash-routed layer (``hash_indices_table`` set), which
+        raises ValueError without them."""
+        topk_weights, topk_ids, local_ids = self._compute_routing(hidden_states, router_logits, gate_weight, input_ids)
         if self.capture_fn is not None:          # logical ids, before any mapping (base_router.py:291-293)
             self.capture_fn(topk_ids)
         self.last_local_ids = local_ids
