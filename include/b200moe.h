@@ -277,6 +277,36 @@ int b200_dsv4_qnorm_rope_kv_insert(void* stream, const void* q, const void* kv, 
                                    const float* cos_sin_cache, int max_position, const int64_t* slot_mapping, void* cache,
                                    int block_size, int num_blocks, int64_t block_stride, void* q_out, int num_tokens,
                                    int num_heads, int q_head_padded, float eps);
+/* DeepSeek-V4 KV compressor (the reference's DeepseekCompressor.forward, models/deepseek_v4/compressor.py), two launches in
+ * stream order.  (head_dim D, compress_ratio R): (512, 4) and (128, 4) with overlapping windows (coff = 2), (512, 128)
+ * without (coff = 1).  kv_score f32 [num_tokens, 2 coff D] (rows kv_score_stride floats apart) = kv | score; ape f32
+ * [R, coff D]; positions, slot_mapping int64 [num_tokens]; state_cache f32 [blocks, state_block_size, 2 coff D], blocks
+ * state_block_stride floats apart.
+ *   state write  token t with s = slot_mapping[t] >= 0: row s of the state = kv | score + ape[position % R];
+ *   compression  token t with s >= 0 and a position p >= 0 with (p + 1) % R == 0: the state rows of positions
+ *                p - (1 + overlap) R + 1 .. p of its request (token_to_req int32 [num_tokens], rows of block_table int32
+ *                [*, block_table_stride] holding state block numbers); positions below 0 are no row.  With overlap the
+ *                older R rows use columns [0, D) of their kv and score halves, the newer R rows [D, 2D).  Per column
+ *                c = sum kv softmax(score) over the rows (fp32); c * rsqrt(mean(c^2) + eps) * w (norm_weight bf16 [D]);
+ *                GPT-J pair RoPE of the last 64 dims at position (p / R) R (clamped to [0, max_position)), cos_sin_cache
+ *                f32 [max_position, 64] = cos | sin; the row goes to slot kv_slot_mapping[t] (int64; < 0 or past the cache:
+ *                nothing written) of kv_cache, blocks block_stride bytes apart:
+ *                  D 512: the 584-byte row of b200_dsv4_qnorm_rope_kv_insert (every value rounded to bf16, NoPE dims
+ *                         per 64 to e4m3 with a ue8m0 scale byte, rope dims bf16);
+ *                  D 128: the 132-byte row of the indexer cache (block_size x 128 e4m3 bytes, then block_size fp32
+ *                         scales): every value rounded to bf16, one scale 2^ceil(log2(max(amax, 1e-4) / 448)).
+ * A window reads the rows the state write of the same call wrote.  No allocation, no synchronisation (graph-capturable).
+ * B200_ERR_INVALID, nothing launched: another (head_dim, compress_ratio), a NULL or misaligned pointer (kv_score, ape,
+ * state_cache, norm_weight, kv_cache 16 bytes; int64 arrays 8; int32 arrays and cos_sin_cache 4), kv_score_stride below
+ * 2 coff D or not a multiple of 4, a state block stride below state_block_size * 2 coff D or not a multiple of 4, a cache
+ * block stride below block_size * 584 (132) bytes or not a multiple of 16 (4), a block size or block count below 1,
+ * max_position < 1, eps < 0 or NaN, num_tokens outside [0, 2^20].  num_tokens 0 launches nothing. */
+int b200_dsv4_compress(void* stream, const float* kv_score, int64_t kv_score_stride, const float* ape,
+                       const int64_t* positions, const int64_t* slot_mapping, const int32_t* token_to_req,
+                       const int32_t* block_table, int64_t block_table_stride, float* state_cache, int state_block_size,
+                       int64_t state_block_stride, const void* norm_weight, float eps, const float* cos_sin_cache,
+                       int max_position, const int64_t* kv_slot_mapping, void* kv_cache, int block_size, int num_blocks,
+                       int64_t block_stride, int head_dim, int compress_ratio, int num_tokens);
 /* DeepSeek-V4 manifold hyper-connections (mHC) for decode, hc_mult = 4 (the reference's mhc_pre / mhc_post /
  * mhc_fused_post_pre / hc_head, vllm/model_executor/kernels/mhc/torch.py:6-106, tilelang_kernels.py:305-350, 884-977).
  * residual bf16 [T, 4, H], x bf16 [T, H], post_layer_mix f32 [T, 4], comb_res_mix f32 [T, 4, 4] (comb[i][j] maps stream i to

@@ -73,6 +73,8 @@ PROTOTYPES = {
                                        _vp, _i32, _vp, _vp, _f32, _i32, _vp, _vp]),
     "b200_dsv4_qnorm_rope_kv_insert": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i64, _vp, _i32, _i32, _i32,
                                               _f32]),
+    "b200_dsv4_compress": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _i64, _vp, _f32, _vp, _i32, _vp,
+                                  _vp, _i32, _i32, _i64, _i32, _i32, _i32]),
     "b200_mla_rope_cache_write": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _f32, _i32, _i32]),
     "b200_mla_q_absorb": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32]),
     "b200_mla_decode_vup": (_i32, [_vp, _vp, _vp, _i32, _vp, _i32, _f32, _f32, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _i32,

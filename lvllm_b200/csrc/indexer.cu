@@ -20,6 +20,7 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "kv_pack.cuh"
 #include "moe_internal.cuh"
 
 namespace cg = cooperative_groups;
@@ -92,29 +93,23 @@ __global__ void __launch_bounds__(IDX_AUX_WARPS * 32)
       }
     }
   }
+  if (is_k) {   // the values are bf16 already, so the packer's rounding leaves them as they are
+    indexer_pack_row132(x, k_ue8m0 != 0, k_cache + (slot / block_size) * (int64_t)block_size * IDX_ROW, block_size,
+                        (int)(slot % block_size), lane);
+    return;
+  }
   float amax = 0.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) amax = fmaxf(amax, fabsf(x[i]));
   amax = warp_max(amax);
-  if (!is_k) {
-    // q_scale = exp2(ceil(log2(max(amax, 1e-10) * (1 / 448)))), always ue8m0; x / q_scale is exact
-    const float sc = ue8m0_ceil(__fmul_rn(fmaxf(amax, 1e-10f), 1.0f / 448.0f));
-    const uint32_t v = e4m3x4(__fdiv_rn(x[0], sc), __fdiv_rn(x[1], sc), __fdiv_rn(x[2], sc), __fdiv_rn(x[3], sc));
-    *reinterpret_cast<uint32_t*>(q_fp8 + ((size_t)t * H + h) * IDX_DIM + lane * 4) = v;
-    if (lane == 0) {
-      const float wt = __bfloat162float(weights[(size_t)t * w_stride + h]);
-      weights_out[(size_t)t * H + h] = __fmul_rn(__fmul_rn(__fmul_rn(wt, sc), softmax_scale), head_scale);
-    }
-    return;
-  }
-  // scale = max(amax, 1e-4) / 448, its power-of-two ceiling when ue8m0; byte = e4m3(k / scale), saturating
-  float sc = __fdiv_rn(fmaxf(amax, 1e-4f), 448.0f);
-  if (k_ue8m0) sc = ue8m0_ceil(sc);
+  // q_scale = exp2(ceil(log2(max(amax, 1e-10) * (1 / 448)))), always ue8m0; x / q_scale is exact
+  const float sc = ue8m0_ceil(__fmul_rn(fmaxf(amax, 1e-10f), 1.0f / 448.0f));
   const uint32_t v = e4m3x4(__fdiv_rn(x[0], sc), __fdiv_rn(x[1], sc), __fdiv_rn(x[2], sc), __fdiv_rn(x[3], sc));
-  uint8_t* blk = k_cache + (slot / block_size) * (int64_t)block_size * IDX_ROW;
-  const int off = (int)(slot % block_size);
-  *reinterpret_cast<uint32_t*>(blk + (size_t)off * IDX_DIM + lane * 4) = v;
-  if (lane == 0) *reinterpret_cast<float*>(blk + (size_t)block_size * IDX_DIM + off * 4) = sc;
+  *reinterpret_cast<uint32_t*>(q_fp8 + ((size_t)t * H + h) * IDX_DIM + lane * 4) = v;
+  if (lane == 0) {
+    const float wt = __bfloat162float(weights[(size_t)t * w_stride + h]);
+    weights_out[(size_t)t * H + h] = __fmul_rn(__fmul_rn(__fmul_rn(wt, sc), softmax_scale), head_scale);
+  }
 }
 
 // ----------------------------------------------------------------------------------------------------------- logits

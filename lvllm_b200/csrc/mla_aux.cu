@@ -18,6 +18,7 @@
 #include <cfloat>
 
 #include "common.cuh"
+#include "kv_pack.cuh"
 #include "moe_internal.cuh"
 
 namespace b200 {
@@ -305,46 +306,19 @@ __global__ void __launch_bounds__(256)
         x[2 * p + 1] = fmaf(e, sn[p], o * cs[p]);
       }
     }
+    if (is_kv) {   // the NoPE values are bf16 already, so the packer's rounding leaves them as they are
+      dsv4_pack_row584(x, cache + (size_t)(slot / block_size) * (size_t)block_stride, block_size, (int)(slot % block_size),
+                       lane);
+      continue;
+    }
     uint32_t pk[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const __nv_bfloat162 b2 = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
       pk[i] = *reinterpret_cast<const uint32_t*>(&b2);
     }
-    if (!is_kv) {
-      *reinterpret_cast<uint4*>(qo) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      *reinterpret_cast<uint4*>(qo + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-      continue;
-    }
-    uint8_t* blk = cache + (size_t)(slot / block_size) * (size_t)block_stride;
-    const int p_in = (int)(slot % block_size);
-    uint8_t* row = blk + (size_t)p_in * 576;
-    if (rope) {
-      *reinterpret_cast<uint4*>(row + 448 + (d0 - 448) * 2) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      *reinterpret_cast<uint4*>(row + 448 + (d0 - 448) * 2 + 16) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-    }
-    // NoPE values are bf16 already: the quantised block is a quad of lanes
-    float amax = 0.f;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) amax = fmaxf(amax, fabsf(x[i]));
-    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-    if (!rope) {
-      const uint32_t e = __float_as_uint(ue8m0_ceil(__fdiv_rn(fmaxf(amax, 1e-4f), 448.f))) >> 23;   // ue8m0 byte
-      const float inv = __uint_as_float((254u - e) << 23);                                            // 1 / scale, exact
-      uint32_t o[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i] * inv, x[4 * i + 1] * inv), __NV_SATFINITE, __NV_E4M3);
-        const uint32_t hi =
-            __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i + 2] * inv, x[4 * i + 3] * inv), __NV_SATFINITE, __NV_E4M3);
-        o[i] = lo | (hi << 16);
-      }
-      *reinterpret_cast<uint4*>(row + d0) = make_uint4(o[0], o[1], o[2], o[3]);
-      uint8_t* srec = blk + (size_t)block_size * 576 + (size_t)p_in * 8;
-      if ((lane & 3) == 0) srec[lane >> 2] = (uint8_t)e;
-      if (lane == 0) srec[7] = 0;
-    }
+    *reinterpret_cast<uint4*>(qo) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+    *reinterpret_cast<uint4*>(qo + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
   }
 }
 

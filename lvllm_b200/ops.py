@@ -428,6 +428,69 @@ def dsv4_qnorm_rope_kv_insert(q: torch.Tensor, kv: torch.Tensor, positions: torc
     return q_out
 
 
+def dsv4_compress(kv_score: torch.Tensor, ape: torch.Tensor, positions: torch.Tensor, state_cache: torch.Tensor,
+                  slot_mapping: torch.Tensor, token_to_req: torch.Tensor, block_table: torch.Tensor,
+                  norm_weight: torch.Tensor, eps: float, cos_sin_cache: torch.Tensor, kv_cache: torch.Tensor,
+                  kv_slot_mapping: torch.Tensor, compress_ratio: int) -> None:
+    """The DeepSeek-V4 KV compressor (the reference's DeepseekCompressor.forward): the state write, then for every token
+    that closes a window of ``compress_ratio`` positions the softmax-pooled compression of the window, RMSNorm, GPT-J RoPE
+    of the last 64 dims and the fp8 store.  D = norm_weight.numel(); coff = 2 (overlapping windows) for ratio 4, 1 for 128.
+    kv_score f32 [T, 2 coff D] = kv | score (the fused wkv / wgate GEMM output; rows may be strided); ape f32 [ratio, coff D];
+    positions [T]; state_cache f32 [blocks, state_block_size, 2 coff D], slot_mapping [T] its slots (< 0: nothing written);
+    token_to_req [T] rows of block_table [*, max_blocks] (state block numbers); norm_weight bf16 [D]; cos_sin_cache f32
+    [max_pos, 64] = cos | sin.  kv_cache, written at kv_slot_mapping[t] (< 0 or past the cache: nothing written): uint8
+    [blocks, block_size, 584] (ops.dsv4_sparse_decode's cache) for D 512 at ratio 4 or 128, uint8 [blocks, block_size, 132]
+    (ops.indexer_logits' cache) for D 128 at ratio 4.  Both caches are written in place; returns None."""
+    ratio = int(compress_ratio)
+    if norm_weight.dtype != torch.bfloat16 or norm_weight.dim() != 1:
+        raise ValueError(f"norm_weight must be bf16 [head_dim], got {norm_weight.dtype} {tuple(norm_weight.shape)}")
+    D = norm_weight.shape[0]
+    row = kv_cache.shape[-1] if kv_cache.dim() == 3 else None
+    if (D, ratio, row) not in ((512, 4, 584), (512, 128, 584), (128, 4, 132)):
+        raise ValueError(f"dsv4_compress runs head_dim 512 at ratio 4 or 128 into a [blocks, block_size, 584] cache and "
+                         f"head_dim 128 at ratio 4 into a [blocks, block_size, 132] cache; got head_dim {D}, ratio {ratio}, "
+                         f"kv_cache {tuple(kv_cache.shape)}")
+    if kv_cache.dtype != torch.uint8 or kv_cache.stride(2) != 1 or kv_cache.stride(1) != row:
+        raise ValueError(f"kv_cache must be uint8 [blocks, block_size, {row}] with rows of {row} contiguous bytes, "
+                         f"got {kv_cache.dtype} strides {kv_cache.stride()}")
+    half = (2 if ratio == 4 else 1) * D
+    T = kv_score.shape[0] if kv_score.dim() == 2 else -1
+    if kv_score.dtype != torch.float32 or T < 0 or kv_score.shape[1] != 2 * half or kv_score.stride(1) != 1:
+        raise ValueError(f"kv_score must be f32 [tokens, {2 * half}] with contiguous rows, got {kv_score.dtype} "
+                         f"{tuple(kv_score.shape)}")
+    if ape.dtype != torch.float32 or tuple(ape.shape) != (ratio, half):
+        raise ValueError(f"ape must be f32 [{ratio}, {half}], got {ape.dtype} {tuple(ape.shape)}")
+    if state_cache.dtype != torch.float32 or state_cache.dim() != 3 or state_cache.shape[2] != 2 * half \
+            or state_cache.stride(2) != 1 or state_cache.stride(1) != 2 * half:
+        raise ValueError(f"state_cache must be f32 [blocks, block_size, {2 * half}] with contiguous rows, got "
+                         f"{state_cache.dtype} {tuple(state_cache.shape)} strides {state_cache.stride()}")
+    if block_table.dim() != 2 or block_table.stride(1) != 1 or block_table.dtype not in (torch.int32, torch.int64):
+        raise ValueError(f"block_table must be int [requests, max_blocks] with contiguous rows, got {block_table.dtype} "
+                         f"{tuple(block_table.shape)}")
+    if cos_sin_cache.dtype != torch.float32 or cos_sin_cache.dim() != 2 or cos_sin_cache.shape[1] != 64:
+        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cos_sin_cache.dtype} {tuple(cos_sin_cache.shape)}")
+    for name, v in (("positions", positions), ("slot_mapping", slot_mapping), ("token_to_req", token_to_req),
+                    ("kv_slot_mapping", kv_slot_mapping)):
+        if v.numel() != T:
+            raise ValueError(f"{name} needs one entry per token ({T}), got {v.numel()}")
+    if T == 0:
+        return
+    ks, sc, kc = kv_score, state_cache, kv_cache   # written or read in place, through their strides
+    if not ks.is_cuda or not sc.is_cuda or not kc.is_cuda:
+        raise ValueError("kv_score, state_cache and kv_cache must be CUDA tensors (lvllm_b200 has no CPU path)")
+    w, cs, ap = _cuda(norm_weight, "norm_weight"), _cuda(cos_sin_cache, "cos_sin_cache"), _cuda(ape, "ape")
+    bt = _i32(block_table, "block_table")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    sm = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
+    ksm = _cuda(kv_slot_mapping.reshape(-1).to(torch.int64), "kv_slot_mapping")
+    req = _i32(token_to_req.reshape(-1), "token_to_req")
+    rc = L.lib().b200_dsv4_compress(
+        _stream(), ks.data_ptr(), ks.stride(0) if T > 1 else 2 * half, ap.data_ptr(), pos.data_ptr(), sm.data_ptr(),
+        req.data_ptr(), bt.data_ptr(), bt.stride(0), sc.data_ptr(), sc.shape[1], sc.stride(0), w.data_ptr(), float(eps),
+        cs.data_ptr(), cs.shape[0], ksm.data_ptr(), kc.data_ptr(), kc.shape[1], kc.shape[0], kc.stride(0), D, ratio, T)
+    L.check(rc, "b200_dsv4_compress")
+
+
 def _mhc_streams(residual: torch.Tensor, name: str = "residual"):
     """bf16 [..., 4, H] -> (contiguous tensor, leading shape, T, H)."""
     r = _cuda(residual, name)
