@@ -397,6 +397,61 @@ int b200_indexer_logits(void* stream, const void* q_fp8, const float* weights, c
                         int num_heads, int max_pages, float* logits, int64_t logits_stride);
 int b200_indexer_topk(void* stream, const float* logits, int64_t logits_stride, int64_t row_width, const int32_t* seq_lens,
                       int batch, int q_len, int topk, int32_t* out);
+/* The C4A indexer of DeepSeek-V4 layers for decode: it picks the compressed keys a token attends to, over the indexer's
+ * 132-byte cache that b200_dsv4_compress writes (head dim 128 at ratio 4; layout as above).  Graph-capturable, no
+ * allocation, no synchronisation; a bad argument returns B200_ERR_INVALID and launches nothing.
+ *
+ *  b200_dsv4_indexer_q_quant  replaces the fp8 path of the reference's _fused_indexer_q_rope_quant_kernel
+ *      (models/deepseek_v4/common/ops/fused_indexer_q.py:70-176).  q bf16 [T,H,128] contiguous = [64 nope | 64 rope],
+ *      weights bf16 [T, >= H] with row stride weights_row_stride elements, positions i64 [T] (clamped to the table),
+ *      cos_sin_cache f32 [max_position, 64] = cos | sin (b200_dsv4_compress's table).  Per (token, head): GPT-J pair RoPE
+ *      of dims 64-127 (pair (64 + 2i, 65 + 2i) with cos[i], sin[i]; fp32 products and sum, no FMA, one bf16 rounding);
+ *      scale = 2^ceil(log2(max(amax, 1e-4) / 448)) over the 128 values (nope as loaded, rope after rounding); q_fp8
+ *      e4m3 [T,H,128] = x / scale, saturating; weights_out f32 [T,H] = w * scale * softmax_scale * head_scale.  No k row.
+ *      1 <= num_heads <= 128, 0 <= num_tokens <= 2^20; q and q_fp8 16-byte aligned.
+ *  b200_dsv4_indexer_decode  the indexer's logits and top-k with one row per token (the reference's
+ *      SparseAttnIndexer decode over the compressed cache).  Token t has n_t = (positions[t] + 1) / compress_ratio
+ *      candidates (0 for positions < 0), at most max_blocks * page_size; its pages are row token_to_req[t] of
+ *      block_table i32 [*, max_blocks] (contiguous).  q_fp8 / weights as b200_dsv4_indexer_q_quant wrote them.  logits f32
+ *      [T, logits_stride] (logits_stride >= max_blocks * page_size): logits[t, j] for j < n_t as b200_indexer_logits
+ *      computes them, -inf to the end of the token's last page.  out i32 [T, topk] = the positions of the topk largest
+ *      logits of [0, n_t), ascending, ties to the lowest positions, -1 padding; n_t <= topk gives 0 .. n_t - 1.
+ *      max_seq_len > 0 promises every positions[t] < max_seq_len: when max_seq_len / compress_ratio <= topk no logit is
+ *      computed (logits untouched) and out is the same.  num_heads 32 or 64, page_size 16, 32 or 64, compress_ratio 4 or
+ *      128, 1 <= topk <= 2048, 0 <= num_tokens <= 2^20; q_fp8 and k_cache 16-byte aligned. */
+int b200_dsv4_indexer_q_quant(void* stream, const void* q, const void* weights, int64_t weights_row_stride,
+                              const int64_t* positions, const float* cos_sin_cache, int max_position, float softmax_scale,
+                              float head_scale, void* q_fp8, float* weights_out, int num_tokens, int num_heads);
+int b200_dsv4_indexer_decode(void* stream, const void* q_fp8, const float* weights, const void* k_cache, int num_blocks,
+                             int page_size, const int64_t* positions, const int32_t* token_to_req,
+                             const int32_t* block_table, int max_blocks, int compress_ratio, int num_tokens,
+                             int num_heads, int64_t max_seq_len, float* logits, int64_t logits_stride, int topk,
+                             int32_t* out);
+/* Global key lists of DeepSeek-V4 decode: what b200_dsv4_sparse_decode (swa / extra indices and lengths) and
+ * b200_dsv4_compress (kv_slot_mapping) take.  One launch; graph-capturable.  Token t has position p = positions[t] and
+ * request row token_to_req[t] of block_table i32 [*, block_table_stride] (the first max_blocks columns used); local index i
+ * of the request is global slot block_table[req][i / block_size] * block_size + i % block_size, and -1 (no key) when
+ * i / block_size >= max_blocks.  A token with slot_mapping[t] < 0 gets length 0 and a row of -1, and its request row is not
+ * read.  out i32 [T, out_stride] (width columns written) and lens i32 [T] for the lists:
+ *   kind 0 SWA            (_compute_swa_indices_and_lens_kernel) param = window W, 1 <= W <= width: keys
+ *                         [max(p - W + 1, 0), p] of the SWA cache's table, length p + 1 - start (0 for p < 0);
+ *   kind 1 C128A          (_build_c128a_topk_metadata_kernel, decode) param = compress_ratio 4 or 128: compressed rows
+ *                         [0, min((p + 1) / ratio, width)) (p < 0: none);
+ *   kind 2 top-k → global (_compute_global_topk_indices_and_lens_kernel) local_topk i32 [T, local_stride >= width], the
+ *                         request-local output of b200_dsv4_indexer_decode: entry j -> its global slot (-1 stays -1),
+ *                         length = the count of entries >= 0;
+ * entries past a list's length are -1.
+ *   kind 3 slot mapping   (_compressed_slot_mapping_kernel) param = compress_ratio 4 or 128: out i64 [T] = the global slot
+ *                         of compressed row p / ratio when p >= 0 and (p + 1) % ratio == 0, else -1; lens, width and
+ *                         out_stride are not used.
+ * B200_ERR_INVALID, nothing launched: another kind, a NULL or misaligned pointer (int64 arrays 8 bytes, int32 4;
+ * positions may be NULL for kind 2),
+ * max_blocks < 1 or > block_table_stride, block_size < 1, num_tokens outside [0, 2^20], for the lists width outside
+ * [1, min(out_stride, 2^20)], and the kind's parameter out of range. */
+int b200_dsv4_indices(void* stream, int kind, const int64_t* positions, const int64_t* slot_mapping,
+                      const int32_t* token_to_req, const int32_t* block_table, int64_t block_table_stride, int max_blocks,
+                      int block_size, int param, const int32_t* local_topk, int64_t local_stride, void* out,
+                      int64_t out_stride, int width, int32_t* lens, int num_tokens);
 /* Paged GQA decode.  q [B,Hq,D] bf16, k_cache/v_cache [num_pages,page_size,Hkv,D] bf16 (contiguous), D=128;
  * out bf16 [B,Hq,D], lse f32 [B,Hq] or NULL. */
 int64_t b200_gqa_decode_workspace_bytes(int batch, int num_q_heads, int head_dim, int num_splits);

@@ -83,6 +83,11 @@ PROTOTYPES = {
                                                       _f32, _f32, _vp, _vp, _i32, _i32]),
     "b200_indexer_logits": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i64]),
     "b200_indexer_topk": (_i32, [_vp, _vp, _i64, _i64, _vp, _i32, _i32, _i32, _vp]),
+    "b200_dsv4_indexer_q_quant": (_i32, [_vp, _vp, _vp, _i64, _vp, _vp, _i32, _f32, _f32, _vp, _vp, _i32, _i32]),
+    "b200_dsv4_indexer_decode": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i64, _vp,
+                                        _i64, _i32, _vp]),
+    "b200_dsv4_indices": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _i32, _vp,
+                                 _i32]),
     "b200_gqa_decode_workspace_bytes": (_i64, [_i32, _i32, _i32, _i32]),
     "b200_gqa_decode": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _f32, _i32,
                                _vp, _vp, _vp]),

@@ -13,6 +13,9 @@
 //                                       lowest positions, -1 padding.
 // Cache layout (indexer_k_quant_and_cache): uint8 [num_blocks, block_size, 132]: a block holds block_size x 128 e4m3 bytes,
 // then block_size fp32 scales (quant_block_size = head_dim = 128: one scale per row).
+// DeepSeek-V4's C4A indexer reuses the logits and top-k kernels with per-token rows (ROWS): row t is one decode token with
+// (positions[t] + 1) / ratio candidate keys in row token_to_req[t] of the compressed cache's block table; its q side is
+// dsv4_indexer_q_quant_kernel (the reference's _fused_indexer_q_rope_quant_kernel, fused_indexer_q.py:70-176, fp8 path).
 #include <cooperative_groups.h>
 #include <cuda.h>
 
@@ -112,6 +115,56 @@ __global__ void __launch_bounds__(IDX_AUX_WARPS * 32)
   }
 }
 
+// The V4 q side, a kernel of its own: V4 rotates the last 64 dims GPT-J style (both dims of a pair sit in one lane, so
+// nothing goes through shared memory), reads an f32 cos | sin table, takes scale = 2^ceil(log2(max(amax, 1e-4) / 448)) and
+// writes no k row; as branches of indexer_qk_rope_quant_cache_kernel those differences would reach every part of it.
+// grid = ceil(T * H / 4) warps of 32, warp w is head (w / H, w % H); lane l owns dims [4l, 4l + 4), lanes 16-31 the rotary
+// dims.  The rotation is fp32 products, their sum, then one rounding to bf16; as in the V3.2 kernel the explicit _rn
+// operations keep the compiler from contracting them into FMAs, which the reference's Triton kernel may do.
+__global__ void __launch_bounds__(IDX_AUX_WARPS * 32)
+    dsv4_indexer_q_quant_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ weights,
+                                int64_t w_stride, const int64_t* __restrict__ positions, const float* __restrict__ cos_sin,
+                                int max_position, float softmax_scale, float head_scale, uint8_t* __restrict__ q_fp8,
+                                float* __restrict__ weights_out, int T, int H) {
+  const int lane = threadIdx.x & 31;
+  const int w = blockIdx.x * IDX_AUX_WARPS + (threadIdx.x >> 5);
+  if (w >= T * H) return;   // whole warps only
+  const int t = w / H, h = w % H;
+  const uint2 raw = *reinterpret_cast<const uint2*>(q + (size_t)w * IDX_DIM + lane * 4);
+  const __nv_bfloat16* hx = reinterpret_cast<const __nv_bfloat16*>(&raw);
+  float x[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) x[i] = __bfloat162float(hx[i]);
+  if (lane >= 16) {
+    int64_t pos = positions[t];
+    pos = pos < 0 ? 0 : (pos >= max_position ? max_position - 1 : pos);
+    const float* cs = cos_sin + pos * IDX_ROT;
+#pragma unroll
+    for (int i = 0; i < 4; i += 2) {
+      const int p = (lane - 16) * 2 + i / 2;   // pair (64 + 2p, 64 + 2p + 1)
+      const float c = cs[p], s = cs[IDX_ROT / 2 + p], x0 = x[i], x1 = x[i + 1];
+      x[i] = bf16r(__fsub_rn(__fmul_rn(x0, c), __fmul_rn(x1, s)));
+      x[i + 1] = bf16r(__fadd_rn(__fmul_rn(x1, c), __fmul_rn(x0, s)));
+    }
+  }
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) amax = fmaxf(amax, fabsf(x[i]));
+  amax = warp_max(amax);
+  // amax is a bf16 value, so max(amax, 1e-4) / 448 is a power of two or far from one: the exponent ceiling is
+  // exp2(ceil(log2(.))) exactly
+  const float sc = ue8m0_ceil(__fdiv_rn(fmaxf(amax, 1e-4f), 448.0f));
+  const uint32_t v = e4m3x4(__fdiv_rn(x[0], sc), __fdiv_rn(x[1], sc), __fdiv_rn(x[2], sc), __fdiv_rn(x[3], sc));
+  *reinterpret_cast<uint32_t*>(q_fp8 + (size_t)w * IDX_DIM + lane * 4) = v;
+  if (lane == 0) {
+    const float wt = __bfloat162float(weights[(size_t)t * w_stride + h]);
+    weights_out[w] = __fmul_rn(__fmul_rn(__fmul_rn(wt, sc), softmax_scale), head_scale);
+  }
+}
+
+// candidate keys of a V4 decode token at position p: the compressed rows its window closes
+B200_DEVICE int64_t v4_keys(int64_t p, int ratio) { return p < 0 ? 0 : (p + 1) / ratio; }
+
 // ----------------------------------------------------------------------------------------------------------- logits
 constexpr int LG_STAGES = 6;
 constexpr int LG_THREADS = 160;          // warps 0-3: MMA + epilogue warpgroup, warp 4: TMA producer
@@ -128,6 +181,10 @@ struct LogitsArgs {
   float* logits;                 // [B * Q, stride]
   int64_t stride;
   int B, Q, H, page, max_pages, qg, n_qg;
+  // ROWS (V4, Q = 1, B = tokens): row b has v4_keys(positions[b], ratio) keys in page_table row row_req[b]
+  const int64_t* positions;
+  const int32_t* row_req;
+  int ratio;
 };
 
 B200_DEVICE void tma_load_3d(void* smem_dst, const void* tmap, int c0, int c1, int c2, uint64_t* bar) {
@@ -138,7 +195,9 @@ B200_DEVICE void tma_load_3d(void* smem_dst, const void* tmap, int c0, int c1, i
       : "memory");
 }
 
+template <bool ROWS>
 B200_DEVICE int lg_keys(const LogitsArgs& a, int b) {
+  if constexpr (ROWS) return (int)min(v4_keys(a.positions[b], a.ratio), (int64_t)a.max_pages * a.page);
   const int S = a.seq_lens[b];
   return S < 0 ? 0 : min(S, a.max_pages * a.page);
 }
@@ -148,6 +207,7 @@ B200_DEVICE int lg_keys(const LogitsArgs& a, int b) {
 struct LgItem {
   int b, g0, qn, t0, t1, S;
 };
+template <bool ROWS>
 B200_DEVICE LgItem lg_item(const LogitsArgs& a, int item, int run_len) {
   LgItem w;
   const int qgi = item % a.n_qg, rb = item / a.n_qg;
@@ -155,13 +215,13 @@ B200_DEVICE LgItem lg_item(const LogitsArgs& a, int item, int run_len) {
   const int run = rb / a.B;
   w.g0 = qgi * a.qg;
   w.qn = min(a.qg, a.Q - w.g0);
-  w.S = lg_keys(a, w.b);
+  w.S = lg_keys<ROWS>(a, w.b);
   w.t0 = run * run_len;
   w.t1 = min(w.t0 + run_len, (w.S + 63) / 64);
   return w;
 }
 
-template <int N, int H>
+template <int N, int H, bool ROWS>
 __global__ void __launch_bounds__(LG_THREADS) indexer_logits_kernel(const __grid_constant__ LogitsArgs a) {
   constexpr int NT = N / H;   // token slots of the q tile (the last ones zero when the q-group is shorter)
   extern __shared__ uint8_t smem_raw[];
@@ -185,7 +245,7 @@ __global__ void __launch_bounds__(LG_THREADS) indexer_logits_kernel(const __grid
   {
     long long sum = 0, mx = 0;
     for (int b = tid; b < a.B; b += LG_THREADS) {
-      const long long t = (lg_keys(a, b) + 63) / 64;
+      const long long t = (lg_keys<ROWS>(a, b) + 63) / 64;
       sum += t;
       mx = max(mx, t);
     }
@@ -219,9 +279,9 @@ __global__ void __launch_bounds__(LG_THREADS) indexer_logits_kernel(const __grid
     if (!elect_one()) return;
     int it = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const LgItem w = lg_item(a, item, run_len);
+      const LgItem w = lg_item<ROWS>(a, item, run_len);
       const int npages = (w.S + a.page - 1) / a.page;
-      const int32_t* pt = a.page_table + (size_t)w.b * a.max_pages;
+      const int32_t* pt = a.page_table + (size_t)(ROWS ? a.row_req[w.b] : w.b) * a.max_pages;
       for (int t = w.t0; t < w.t1; ++t, ++it) {
         const int s = it % LG_STAGES;
         mbar_wait(&empty[s], ((it / LG_STAGES) & 1) ^ 1);
@@ -243,7 +303,7 @@ __global__ void __launch_bounds__(LG_THREADS) indexer_logits_kernel(const __grid
   const uint32_t qa = smem_u32(qt), ka = smem_u32(kt);
   int it = 0;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-    const LgItem w = lg_item(a, item, run_len);
+    const LgItem w = lg_item<ROWS>(a, item, run_len);
     if (w.t0 >= w.t1) continue;
     const int row0 = w.b * a.Q + w.g0;   // first logits row of the q-group
     // the previous item's MMAs have retired (wait_group 0 after each tile); every thread is past its reads of the q tile
@@ -351,9 +411,12 @@ B200_DEVICE unsigned long long tk_scan(unsigned long long v, unsigned long long*
 // CTA derives the same threshold).  Each CTA's own histograms also give its segment's counts of keys above and equal to
 // the threshold, and one ordered compaction writes the selected positions in ascending order, each CTA at the offset the
 // lower ranks' counts give it.  Row r starts at r * stride; positions past `width` are never read.
-__global__ void __launch_bounds__(TK_THREADS) indexer_topk_kernel(const float* __restrict__ logits, int64_t stride,
-                                                                  int64_t width, const int32_t* __restrict__ seq_lens,
-                                                                  int Q, int topk, int32_t* __restrict__ out) {
+// ROWS (V4, Q = 1): row r has v4_keys(positions[r], ratio) positions; seq_lens is not read.
+template <bool ROWS>
+__global__ void __launch_bounds__(TK_THREADS)
+    indexer_topk_kernel(const float* __restrict__ logits, int64_t stride, int64_t width,
+                        const int32_t* __restrict__ seq_lens, int Q, int topk, int32_t* __restrict__ out,
+                        const int64_t* __restrict__ positions, int ratio) {
   __shared__ int hist[TK_BINS];
   __shared__ int ghist[TK_BINS];
   __shared__ unsigned long long scan_sh[64];
@@ -366,7 +429,7 @@ __global__ void __launch_bounds__(TK_THREADS) indexer_topk_kernel(const float* _
   const int row = blockIdx.x / CS;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = row / Q, i = row % Q;
-  const int64_t n = min((int64_t)max(0, seq_lens[b] - Q + i + 1), width);
+  const int64_t n = min(ROWS ? v4_keys(positions[row], ratio) : (int64_t)max(0, seq_lens[b] - Q + i + 1), width);
   int32_t* o = out + (size_t)row * topk;
   if (n <= topk) {   // every position, in order, then -1
     if (rank == 0)
@@ -509,6 +572,82 @@ static int tm_encode_cache(CUtensorMap* tm, const void* k_cache, int num_blocks,
 
 static bool misaligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 != 0; }
 
+template <int N, int H, bool ROWS>
+static int run_logits(const LogitsArgs& a, int grid, cudaStream_t st) {
+  const int smem = 1024 + N * IDX_DIM + LG_STAGES * (LG_TILE + LG_SCALES);
+  const int rc = kernel_smem(reinterpret_cast<const void*>(indexer_logits_kernel<N, H, ROWS>), smem,
+                             "cudaFuncSetAttribute(indexer_logits)");
+  if (rc) return rc;
+  indexer_logits_kernel<N, H, ROWS><<<grid, LG_THREADS, smem, st>>>(a);
+  return 0;
+}
+
+// Encodes the cache's tensor map, sizes the q-groups and launches indexer_logits_kernel; the caller has checked and
+// filled every other field of a (ROWS: Q = 1, so one token per q tile and N = 64).
+template <bool ROWS>
+static int launch_logits(LogitsArgs& a, int num_blocks, cudaStream_t st, const char* who) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
+  const int sms = device_sms(dev);
+  if (sms < 0) return sms;
+  int rc = tm_encode_cache(&a.tmK, a.k_cache, num_blocks, a.page);
+  if (rc) return rc;
+  a.qg = std::min(a.Q, 128 / a.H);
+  a.n_qg = (a.Q + a.qg - 1) / a.qg;
+  // the kernel sizes its runs of tiles from the rows' key counts; the most items it can make are those of 4-tile runs
+  // over the page table's width
+  const int64_t tiles = ((int64_t)a.max_pages * a.page + 63) / 64;
+  const int64_t items = (tiles + 3) / 4 * a.B * a.n_qg;
+  if (items > 0x7FFFFFFFll) {
+    set_error(std::string(who) + ": too much work for one launch");
+    return B200_ERR_INVALID;
+  }
+  const int grid = (int)std::min<int64_t>(items, 2 * sms);
+  if constexpr (ROWS) rc = a.H == 32 ? run_logits<64, 32, true>(a, grid, st) : run_logits<64, 64, true>(a, grid, st);
+  else if (a.qg * a.H <= 64) rc = a.H == 32 ? run_logits<64, 32, false>(a, grid, st) : run_logits<64, 64, false>(a, grid, st);
+  else rc = a.H == 32 ? run_logits<128, 32, false>(a, grid, st) : run_logits<128, 64, false>(a, grid, st);
+  if (rc) return rc;
+  ++g_launches;
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "indexer_logits launch");
+  return 0;
+}
+
+// rows of the top-k, each on a cluster of CS CTAs while the rows alone would leave most SMs idle
+template <bool ROWS>
+static int launch_topk(const float* logits, int64_t stride, int64_t width, const int32_t* seq_lens, int Q, int topk,
+                       int32_t* out, const int64_t* positions, int ratio, int64_t rows, cudaStream_t st, const char* who) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
+  const int sms = device_sms(dev);
+  if (sms < 0) return sms;
+  int cs = 1;
+  while (cs < 8 && rows * cs * 2 <= sms) cs *= 2;
+  if (rows * cs > 0x7FFFFFFFll) {
+    set_error(std::string(who) + ": too many rows");
+    return B200_ERR_INVALID;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(rows * cs));
+  cfg.blockDim = dim3(TK_THREADS);
+  cfg.dynamicSmemBytes = 0;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cs;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  e = cudaLaunchKernelEx(&cfg, indexer_topk_kernel<ROWS>, logits, stride, width, seq_lens, Q, topk, out, positions, ratio);
+  ++g_launches;
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "indexer_topk launch");
+  return 0;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -573,14 +712,7 @@ int b200_indexer_logits(void* stream, const void* q_fp8, const float* weights, c
     return B200_ERR_INVALID;
   }
   if (batch == 0) return 0;
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
-  const int sms = device_sms(dev);
-  if (sms < 0) return sms;
   LogitsArgs a{};
-  int rc = tm_encode_cache(&a.tmK, k_cache, num_blocks, page_size);
-  if (rc) return rc;
   a.k_cache = reinterpret_cast<const uint8_t*>(k_cache);
   a.q_fp8 = reinterpret_cast<const uint8_t*>(q_fp8);
   a.weights = weights;
@@ -593,33 +725,7 @@ int b200_indexer_logits(void* stream, const void* q_fp8, const float* weights, c
   a.H = num_heads;
   a.page = page_size;
   a.max_pages = max_pages;
-  a.qg = std::min(q_len, 128 / num_heads);
-  a.n_qg = (q_len + a.qg - 1) / a.qg;
-  // the kernel sizes its runs of tiles from seq_lens; the most items it can make are those of 4-tile runs over the
-  // page table's width
-  const int64_t tiles = ((int64_t)max_pages * page_size + 63) / 64;
-  const int64_t items = (tiles + 3) / 4 * batch * a.n_qg;
-  if (items > 0x7FFFFFFFll) {
-    set_error("b200_indexer_logits: too much work for one launch");
-    return B200_ERR_INVALID;
-  }
-  const int N = a.qg * num_heads <= 64 ? 64 : 128;
-  const void* fn = N == 64 ? (num_heads == 32 ? reinterpret_cast<const void*>(indexer_logits_kernel<64, 32>)
-                                              : reinterpret_cast<const void*>(indexer_logits_kernel<64, 64>))
-                           : (num_heads == 32 ? reinterpret_cast<const void*>(indexer_logits_kernel<128, 32>)
-                                              : reinterpret_cast<const void*>(indexer_logits_kernel<128, 64>));
-  const int smem = 1024 + N * IDX_DIM + LG_STAGES * (LG_TILE + LG_SCALES);
-  if ((rc = kernel_smem(fn, smem, "cudaFuncSetAttribute(indexer_logits)"))) return rc;
-  const int grid = (int)std::min<int64_t>(items, 2 * sms);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (N == 64 && num_heads == 32) indexer_logits_kernel<64, 32><<<grid, LG_THREADS, smem, st>>>(a);
-  else if (N == 64) indexer_logits_kernel<64, 64><<<grid, LG_THREADS, smem, st>>>(a);
-  else if (num_heads == 32) indexer_logits_kernel<128, 32><<<grid, LG_THREADS, smem, st>>>(a);
-  else indexer_logits_kernel<128, 64><<<grid, LG_THREADS, smem, st>>>(a);
-  ++g_launches;
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "indexer_logits launch");
-  return 0;
+  return launch_logits<false>(a, num_blocks, reinterpret_cast<cudaStream_t>(stream), "b200_indexer_logits");
 }
 
 int b200_indexer_topk(void* stream, const float* logits, int64_t logits_stride, int64_t row_width, const int32_t* seq_lens,
@@ -635,35 +741,92 @@ int b200_indexer_topk(void* stream, const float* logits, int64_t logits_stride, 
   }
   const int64_t rows = (int64_t)batch * q_len;
   if (rows == 0) return 0;
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
-  const int sms = device_sms(dev);
-  if (sms < 0) return sms;
-  // a cluster of CS CTAs per row while the rows alone would leave most SMs idle
-  int cs = 1;
-  while (cs < 8 && rows * cs * 2 <= sms) cs *= 2;
-  if (rows * cs > 0x7FFFFFFFll) {
-    set_error("b200_indexer_topk: too many rows");
+  return launch_topk<false>(logits, logits_stride, row_width, seq_lens, q_len, topk, out, nullptr, 0, rows,
+                            reinterpret_cast<cudaStream_t>(stream), "b200_indexer_topk");
+}
+
+int b200_dsv4_indexer_q_quant(void* stream, const void* q, const void* weights, int64_t weights_row_stride,
+                              const int64_t* positions, const float* cos_sin_cache, int max_position, float softmax_scale,
+                              float head_scale, void* q_fp8, float* weights_out, int num_tokens, int num_heads) {
+  if (!q || !weights || !positions || !cos_sin_cache || !q_fp8 || !weights_out || num_tokens < 0 ||
+      num_tokens > (1 << 20) || num_heads < 1 || num_heads > 128 || max_position < 1 || weights_row_stride < num_heads) {
+    set_error("b200_dsv4_indexer_q_quant: bad argument (1 <= num_heads <= 128, 0 <= num_tokens <= 2^20, "
+              "weights_row_stride >= num_heads, max_position >= 1)");
     return B200_ERR_INVALID;
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(rows * cs));
-  cfg.blockDim = dim3(TK_THREADS);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = reinterpret_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cs;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, indexer_topk_kernel, logits, logits_stride, row_width, seq_lens, q_len, topk, out);
+  if (misaligned16(q) || misaligned16(q_fp8) || reinterpret_cast<uintptr_t>(weights) % 2 ||
+      reinterpret_cast<uintptr_t>(positions) % 8 || reinterpret_cast<uintptr_t>(cos_sin_cache) % 4 ||
+      reinterpret_cast<uintptr_t>(weights_out) % 4) {
+    set_error("b200_dsv4_indexer_q_quant: q and q_fp8 must be 16-byte aligned, positions 8, cos_sin_cache and "
+              "weights_out 4, weights 2");
+    return B200_ERR_INVALID;
+  }
+  if (num_tokens == 0) return 0;
+  const int64_t warps = (int64_t)num_tokens * num_heads;
+  dsv4_indexer_q_quant_kernel<<<(unsigned)((warps + IDX_AUX_WARPS - 1) / IDX_AUX_WARPS), IDX_AUX_WARPS * 32, 0,
+                                reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(weights), weights_row_stride,
+      positions, cos_sin_cache, max_position, softmax_scale, head_scale, reinterpret_cast<uint8_t*>(q_fp8), weights_out,
+      num_tokens, num_heads);
   ++g_launches;
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "indexer_topk launch");
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "dsv4_indexer_q_quant launch");
   return 0;
+}
+
+int b200_dsv4_indexer_decode(void* stream, const void* q_fp8, const float* weights, const void* k_cache, int num_blocks,
+                             int page_size, const int64_t* positions, const int32_t* token_to_req,
+                             const int32_t* block_table, int max_blocks, int compress_ratio, int num_tokens,
+                             int num_heads, int64_t max_seq_len, float* logits, int64_t logits_stride, int topk,
+                             int32_t* out) {
+  if (!q_fp8 || !weights || !k_cache || !positions || !token_to_req || !block_table || !logits || !out ||
+      num_blocks < 1 || max_blocks < 1 || num_tokens < 0 || num_tokens > (1 << 20)) {
+    set_error("b200_dsv4_indexer_decode: bad argument (NULL pointer, num_blocks or max_blocks < 1, num_tokens outside "
+              "[0, 2^20])");
+    return B200_ERR_INVALID;
+  }
+  if ((num_heads != 32 && num_heads != 64) || (page_size != 16 && page_size != 32 && page_size != 64) ||
+      (compress_ratio != 4 && compress_ratio != 128) || topk < 1 || topk > 2048) {
+    set_error("b200_dsv4_indexer_decode: needs num_heads 32 or 64, page_size 16, 32 or 64, compress_ratio 4 or 128, "
+              "1 <= topk <= 2048");
+    return B200_ERR_INVALID;
+  }
+  const int64_t width = (int64_t)max_blocks * page_size;
+  if (logits_stride < width || logits_stride > 0x7FFFFFFFll) {
+    set_error("b200_dsv4_indexer_decode: logits_stride must be >= max_blocks * page_size and < 2^31");
+    return B200_ERR_INVALID;
+  }
+  if (misaligned16(q_fp8) || misaligned16(k_cache) || reinterpret_cast<uintptr_t>(weights) % 4 ||
+      reinterpret_cast<uintptr_t>(positions) % 8 || reinterpret_cast<uintptr_t>(token_to_req) % 4 ||
+      reinterpret_cast<uintptr_t>(block_table) % 4 || reinterpret_cast<uintptr_t>(logits) % 4 ||
+      reinterpret_cast<uintptr_t>(out) % 4) {
+    set_error("b200_dsv4_indexer_decode: q_fp8 and k_cache must be 16-byte aligned, positions 8, the rest 4");
+    return B200_ERR_INVALID;
+  }
+  if (num_tokens == 0) return 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // every token of a short context selects all of its candidates: the top-k writes them without reading a logit
+  if (max_seq_len <= 0 || max_seq_len / compress_ratio > topk) {
+    LogitsArgs a{};
+    a.k_cache = reinterpret_cast<const uint8_t*>(k_cache);
+    a.q_fp8 = reinterpret_cast<const uint8_t*>(q_fp8);
+    a.weights = weights;
+    a.page_table = block_table;
+    a.logits = logits;
+    a.stride = logits_stride;
+    a.B = num_tokens;
+    a.Q = 1;
+    a.H = num_heads;
+    a.page = page_size;
+    a.max_pages = max_blocks;
+    a.positions = positions;
+    a.row_req = token_to_req;
+    a.ratio = compress_ratio;
+    const int rc = launch_logits<true>(a, num_blocks, st, "b200_dsv4_indexer_decode");
+    if (rc) return rc;
+  }
+  return launch_topk<true>(logits, logits_stride, width, nullptr, 1, topk, out, positions, compress_ratio, num_tokens, st,
+                           "b200_dsv4_indexer_decode");
 }
 
 }  // extern "C"

@@ -849,3 +849,172 @@ def indexer_decode(q_fp8: torch.Tensor, weights: torch.Tensor, k_cache: torch.Te
     positions, the layout mla_decode_sparse takes with req_id = row // q_len and the same page table."""
     logits = indexer_logits(q_fp8, weights, k_cache, seq_lens, page_table, q_len)
     return indexer_topk(logits, seq_lens, topk, q_len)
+
+
+def dsv4_indexer_q_quant(q: torch.Tensor, weights: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.Tensor,
+                         softmax_scale: float, head_scale: float):
+    """The DeepSeek-V4 indexer's q side (the fp8 path of the reference's fused_indexer_q_rope_quant,
+    models/deepseek_v4/common/ops/fused_indexer_q.py:70-176).  q bf16 [T, H, 128] = [64 nope | 64 rope] (wq_b output);
+    weights bf16 [T, H], any row stride (a column slice of the fused projection); positions [T]; cos_sin_cache f32
+    [max_pos, 64] = cos | sin (the table ops.dsv4_compress takes).  Per (token, head): GPT-J pair RoPE of dims 64-127 in
+    fp32, rounded to bf16 once; scale = 2^ceil(log2(max(amax, 1e-4) / 448)); q_fp8 = e4m3(x / scale), saturating.  The model
+    passes softmax_scale = 128 ** -0.5 and head_scale = H ** -0.5.  Returns (q_fp8 e4m3 [T, H, 128], weights_out f32
+    [T, H] = weights * scale * softmax_scale * head_scale), what ops.dsv4_indexer_decode takes."""
+    if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 128 or not 1 <= q.shape[1] <= 128:
+        raise ValueError(f"q must be bf16 [T, 1-128 heads, 128], got {q.dtype} {tuple(q.shape)}")
+    T, H, _ = q.shape
+    if weights.dtype != torch.bfloat16 or weights.shape != (T, H) or weights.stride(1) != 1 \
+            or (T > 1 and weights.stride(0) < H):
+        raise ValueError(f"weights must be a bf16 [{T}, {H}] view with contiguous, non-overlapping rows")
+    if cos_sin_cache.dtype != torch.float32 or cos_sin_cache.dim() != 2 or cos_sin_cache.shape[1] != 64:
+        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cos_sin_cache.dtype} "
+                         f"{tuple(cos_sin_cache.shape)}")
+    if positions.numel() != T:
+        raise ValueError(f"positions needs one entry per token ({T}), got {positions.numel()}")
+    if not weights.is_cuda:
+        raise ValueError("weights must be a CUDA tensor (lvllm_b200 has no CPU path)")
+    x, cs = _cuda(q, "q"), _cuda(cos_sin_cache, "cos_sin_cache")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    q_fp8 = torch.empty(T, H, 128, dtype=torch.float8_e4m3fn, device=x.device)
+    w_out = torch.empty(T, H, dtype=torch.float32, device=x.device)
+    rc = L.lib().b200_dsv4_indexer_q_quant(_stream(), x.data_ptr(), weights.data_ptr(), weights.stride(0) if T > 1 else H,
+                                           pos.data_ptr(), cs.data_ptr(), cs.shape[0], float(softmax_scale),
+                                           float(head_scale), q_fp8.data_ptr(), w_out.data_ptr(), T, H)
+    L.check(rc, "b200_dsv4_indexer_q_quant")
+    return q_fp8, w_out
+
+
+def dsv4_indexer_decode(q_fp8: torch.Tensor, weights: torch.Tensor, k_cache: torch.Tensor, positions: torch.Tensor,
+                        token_to_req: torch.Tensor, block_table: torch.Tensor, compress_ratio: int, topk: int,
+                        max_seq_len: int | None = None, logits: torch.Tensor | None = None) -> torch.Tensor:
+    """The DeepSeek-V4 C4A indexer's decode step: logits then top-k, one row per token.  q_fp8 e4m3 [T, H, 128] and
+    weights f32 [T, H] from ops.dsv4_indexer_q_quant (H 32 or 64); k_cache uint8 [blocks, page, 132] (page 16, 32 or 64),
+    the compressed indexer cache ops.dsv4_compress writes; block_table [requests, max_blocks] its block numbers.  Token t
+    has (positions[t] + 1) // compress_ratio candidates (at most max_blocks * page) in row token_to_req[t].  ``logits``
+    (f32 [T, >= max_blocks * page], contiguous rows) receives the logits when given.  max_seq_len, when given, must be
+    > every position: if max_seq_len // compress_ratio <= topk every token selects all of its candidates and no logit is
+    computed (the reference's short-context path).  Returns the request-local top-k int32 [T, topk], ascending, -1
+    padded; ops.dsv4_global_topk_indices turns it into dsv4_sparse_decode's extra list."""
+    if q_fp8.dtype != torch.float8_e4m3fn or q_fp8.dim() != 3 or q_fp8.shape[2] != 128 or q_fp8.shape[1] not in (32, 64):
+        raise ValueError(f"q_fp8 must be e4m3 [T, 32 or 64, 128], got {q_fp8.dtype} {tuple(q_fp8.shape)}")
+    T, H, _ = q_fp8.shape
+    if weights.dtype != torch.float32 or weights.shape != (T, H):
+        raise ValueError(f"weights must be f32 [{T}, {H}], got {weights.dtype} {tuple(weights.shape)}")
+    if k_cache.dtype != torch.uint8 or k_cache.dim() != 3 or k_cache.shape[2] != 132 or not k_cache.is_contiguous():
+        raise ValueError(f"k_cache must be a contiguous uint8 [num_blocks, page, 132], got {tuple(k_cache.shape)}")
+    if block_table.dim() != 2 or block_table.dtype not in (torch.int32, torch.int64):
+        raise ValueError(f"block_table must be int [requests, max_blocks], got {block_table.dtype} "
+                         f"{tuple(block_table.shape)}")
+    ratio, k = int(compress_ratio), int(topk)
+    if ratio not in (4, 128) or not 1 <= k <= 2048:
+        raise ValueError(f"compress_ratio must be 4 or 128 and topk 1-2048, got {ratio}, {k}")
+    if positions.numel() != T or token_to_req.numel() != T:
+        raise ValueError(f"positions and token_to_req need one entry per token ({T})")
+    page = k_cache.shape[1]
+    width = block_table.shape[1] * page
+    if logits is None:
+        logits = torch.empty(T, width, dtype=torch.float32, device=q_fp8.device)
+    elif logits.dtype != torch.float32 or logits.dim() != 2 or logits.shape[0] != T or logits.shape[1] < width \
+            or logits.stride(1) != 1:
+        raise ValueError(f"logits must be f32 [{T}, >= {width}] with contiguous rows")
+    out = torch.empty(T, k, dtype=torch.int32, device=q_fp8.device)
+    if T == 0:
+        return out
+    q8, w, kc = _cuda(q_fp8, "q_fp8"), _cuda(weights, "weights"), _cuda(k_cache, "k_cache")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    req = _i32(token_to_req.reshape(-1), "token_to_req")
+    bt = _i32(block_table, "block_table")
+    rc = L.lib().b200_dsv4_indexer_decode(
+        _stream(), q8.data_ptr(), w.data_ptr(), kc.data_ptr(), kc.shape[0], page, pos.data_ptr(), req.data_ptr(),
+        bt.data_ptr(), bt.shape[1], ratio, T, H, int(max_seq_len) if max_seq_len is not None else 0, logits.data_ptr(),
+        logits.stride(0) if T > 1 else logits.shape[1], k, out.data_ptr())
+    L.check(rc, "b200_dsv4_indexer_decode")
+    return out
+
+
+_DS_IDX_SWA, _DS_IDX_C128A, _DS_IDX_TOPK, _DS_IDX_SLOTMAP = 0, 1, 2, 3
+
+
+def _dsv4_indices(kind: int, positions, slot_mapping, token_to_req, block_table, block_size: int, param: int,
+                  width: int, local_topk=None):
+    """One b200_dsv4_indices call; returns (indices int32 [T, width], lens int32 [T]), or the int64 [T] slot mapping."""
+    if block_table.dim() != 2 or block_table.dtype not in (torch.int32, torch.int64) or block_table.shape[1] < 1:
+        raise ValueError(f"block_table must be int [requests, max_blocks >= 1], got {block_table.dtype} "
+                         f"{tuple(block_table.shape)}")
+    if int(block_size) < 1:
+        raise ValueError(f"block_size must be >= 1, got {block_size}")
+    T = positions.numel() if local_topk is None else local_topk.shape[0]
+    for name, v in (("positions", positions), ("slot_mapping", slot_mapping), ("token_to_req", token_to_req)):
+        if v is not None and v.numel() != T:
+            raise ValueError(f"{name} needs one entry per token ({T}), got {v.numel()}")
+    dev = block_table.device
+    if kind == _DS_IDX_SLOTMAP:
+        out, lens = torch.empty(T, dtype=torch.int64, device=dev), None
+    else:
+        out = torch.empty(T, width, dtype=torch.int32, device=dev)
+        lens = torch.empty(T, dtype=torch.int32, device=dev)
+    if T == 0:
+        return out if lens is None else (out, lens)
+    bt = _i32(block_table, "block_table")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions") if positions is not None else None
+    sm = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
+    req = _i32(token_to_req.reshape(-1), "token_to_req")
+    loc = _i32(local_topk, "topk_indices") if local_topk is not None else None
+    rc = L.lib().b200_dsv4_indices(
+        _stream(), kind, pos.data_ptr() if pos is not None else None, sm.data_ptr(), req.data_ptr(), bt.data_ptr(), bt.stride(0), bt.shape[1],
+        int(block_size), int(param), loc.data_ptr() if loc is not None else None, loc.shape[1] if loc is not None else 0,
+        out.data_ptr(), width, width, lens.data_ptr() if lens is not None else None, T)
+    L.check(rc, "b200_dsv4_indices")
+    return out if lens is None else (out, lens)
+
+
+def dsv4_swa_indices(positions: torch.Tensor, slot_mapping: torch.Tensor, token_to_req: torch.Tensor,
+                     block_table: torch.Tensor, block_size: int, window: int):
+    """Sliding-window key list of DeepSeek-V4 decode (the reference's _compute_swa_indices_and_lens_kernel, with p taken
+    from positions): token t at position p attends to positions [max(p - window + 1, 0), p] of its request, as global
+    slots of the SWA cache: block_table[token_to_req[t]][i // block_size] * block_size + i % block_size (block_table
+    [requests, max_blocks]; a block column >= max_blocks is no key, -1).  A token with slot_mapping < 0 gets length 0.
+    Returns (swa_indices int32 [T, window], -1 past the length; swa_lens int32 [T]), what ops.dsv4_sparse_decode takes."""
+    if int(window) < 1:
+        raise ValueError(f"window must be >= 1, got {window}")
+    return _dsv4_indices(_DS_IDX_SWA, positions, slot_mapping, token_to_req, block_table, block_size, window, int(window))
+
+
+def dsv4_c128a_indices(positions: torch.Tensor, slot_mapping: torch.Tensor, token_to_req: torch.Tensor,
+                       block_table: torch.Tensor, block_size: int, compress_ratio: int, width: int):
+    """Compressed key list of a DeepSeek-V4 C128A layer for decode (the decode branch of the reference's
+    _build_c128a_topk_metadata_kernel): every compressed row [0, min((p + 1) // compress_ratio, width)) of the token's
+    request, as global slots of the compressed cache (block_table [requests, max_blocks] of the compressed cache, whose
+    block size is block_size; a block column >= max_blocks is no key, -1).  A token with slot_mapping < 0 gets length 0.
+    Returns (extra_indices int32 [T, width], -1 past the length; extra_lens int32 [T])."""
+    if int(compress_ratio) not in (4, 128) or int(width) < 1:
+        raise ValueError(f"compress_ratio must be 4 or 128 and width >= 1, got {compress_ratio}, {width}")
+    return _dsv4_indices(_DS_IDX_C128A, positions, slot_mapping, token_to_req, block_table, block_size, compress_ratio,
+                         int(width))
+
+
+def dsv4_global_topk_indices(topk_indices: torch.Tensor, slot_mapping: torch.Tensor, token_to_req: torch.Tensor,
+                             block_table: torch.Tensor, block_size: int):
+    """Request-local C4A top-k (ops.dsv4_indexer_decode's output, int [T, topk]) -> global slots of the compressed
+    attention cache (the reference's compute_global_topk_indices_and_lens): entry i >= 0 becomes
+    block_table[token_to_req[t]][i // block_size] * block_size + i % block_size (a block column >= max_blocks: -1), -1
+    stays -1; the length is the count of entries >= 0, 0 for a token with slot_mapping < 0.
+    Returns (extra_indices int32 [T, topk]; extra_lens int32 [T])."""
+    if topk_indices.dim() != 2 or topk_indices.dtype not in (torch.int32, torch.int64) or topk_indices.shape[1] < 1:
+        raise ValueError(f"topk_indices must be int [tokens, topk >= 1], got {topk_indices.dtype} "
+                         f"{tuple(topk_indices.shape)}")
+    return _dsv4_indices(_DS_IDX_TOPK, None, slot_mapping, token_to_req, block_table, block_size, 0,
+                         topk_indices.shape[1], local_topk=topk_indices)
+
+
+def dsv4_compressed_slot_mapping(positions: torch.Tensor, slot_mapping: torch.Tensor, token_to_req: torch.Tensor,
+                                 block_table: torch.Tensor, block_size: int, compress_ratio: int) -> torch.Tensor:
+    """The compressor's cache slots (the reference's get_compressed_slot_mapping): a token at position p that closes a
+    window ((p + 1) % compress_ratio == 0) writes compressed row p // compress_ratio of its request, global slot
+    block_table[token_to_req[t]][row // block_size] * block_size + row % block_size of the compressed cache; every other
+    token, a token with slot_mapping < 0 and a block column >= max_blocks get -1.  Returns int64 [T], the kv_slot_mapping
+    ops.dsv4_compress takes."""
+    if int(compress_ratio) not in (4, 128):
+        raise ValueError(f"compress_ratio must be 4 or 128, got {compress_ratio}")
+    return _dsv4_indices(_DS_IDX_SLOTMAP, positions, slot_mapping, token_to_req, block_table, block_size, compress_ratio,
+                         1)
