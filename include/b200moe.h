@@ -452,6 +452,40 @@ int b200_dsv4_indices(void* stream, int kind, const int64_t* positions, const in
                       const int32_t* token_to_req, const int32_t* block_table, int64_t block_table_stride, int max_blocks,
                       int block_size, int param, const int32_t* local_topk, int64_t local_stride, void* out,
                       int64_t out_stride, int width, int32_t* lens, int num_tokens);
+/* The DeepSeek-V4 attention output projection's first two steps (the reference's deep_gemm_fp8_o_proj,
+ * models/deepseek_v4/nvidia/ops/o_proj.py:28-73; wo_b stays with the caller).  G = n_groups, heads_per_group hpg = H / G,
+ * D = hpg * 512, R = o_lora_rank.  One launch each, no allocation, no synchronisation: graph-capturable.  A bad argument
+ * returns B200_ERR_INVALID and launches nothing; num_tokens 0 launches nothing.
+ *
+ *  b200_dsv4_inv_rope_quant  replaces fused_inv_rope_fp8_quant, fp32-scale path (common/ops/fused_inv_rope_fp8_quant.py).
+ *      o bf16 [T, H, 512] = [448 nope | 64 rope], heads and dims contiguous, token stride o_token_stride elements (>= H * 512,
+ *      a multiple of 8); positions i64 [T] (clamped to the table); cos_sin_cache f32 [max_position, 64] = cos | sin
+ *      (b200_dsv4_qnorm_rope_kv_insert's table).  Per (token, head): the inverse GPT-J pair rotation of dims 448-511, pair
+ *      (448 + 2i, 449 + 2i) = (x, y) -> (x cos[i] + y sin[i], y cos[i] - x sin[i]) in fp32, products and sum rounded
+ *      separately (no FMA), not rounded to bf16.  Per 128 values of a group (a head's dims [128 b, 128 b + 128)):
+ *      scale = 2^ceil(log2(max(absmax, 1e-10) * (1 / 448))), the ceiling taken exactly from the fp32 bits of the product;
+ *      codes = e4m3(clamp(x / scale, -448, 448)), round to nearest even.  Outputs in this module's layout:
+ *      o_fp8 e4m3 [G][T][D] (element (t, g, d) at (g * T + t) * D + d) and o_scale f32 [G][D / 128][T] (element (t, g, b)
+ *      at (g * D / 128 + b) * T + t).  0 <= num_tokens <= 2^20, 1 <= hpg <= 16; o and o_fp8 16-byte aligned.
+ *  b200_dsv4_wo_a_workspace_bytes  workspace b200_dsv4_wo_a needs on the current device (0: none).  A workspace sized for
+ *      some T serves every smaller T of every shape; its first bytes hold arrival counters that must be zero before the
+ *      first call and that every call leaves zero.
+ *  b200_dsv4_wo_a  replaces DeepGEMM's fp8_einsum("bhr,hdr->bhd") with recipe (1, 128, 128): z bf16 [T, G * R],
+ *      z[t, g * R + r] = sum over k-blocks kb of (sum_k o_fp8[t, g, 128 kb + k] * wo_a[g * R + r, 128 kb + k]) *
+ *      wo_a_scale[(g * R + r) / 128, kb] * o_scale[t, g, kb], the inner sum one tensor-core accumulation, the outer in fp32,
+ *      rounded to bf16 once.  o_fp8 / o_scale as b200_dsv4_inv_rope_quant wrote them; wo_a e4m3 [G * R, D] row-major (the
+ *      checkpoint tensor, read in place); wo_a_scale f32 [G * R / 128, D / 128] (checkpoints that store e8m0 scales convert
+ *      them to f32 once: exact).  K is split over CTAs by G, R, D and the SM count, never by T, and the splits are added in
+ *      fixed order: z of a token does not depend on the other tokens of the call, and repeated calls give the same bits.
+ *      0 <= num_tokens <= 2^20, n_groups >= 1, heads_per_group 1-16, o_lora_rank a multiple of 128, G * R / 64 <= 65535;
+ *      o_fp8, wo_a and workspace 16-byte aligned. */
+int b200_dsv4_inv_rope_quant(void* stream, const void* o, int64_t o_token_stride, const int64_t* positions,
+                             const float* cos_sin_cache, int max_position, int num_tokens, int num_heads, int n_groups,
+                             void* o_fp8, float* o_scale);
+int64_t b200_dsv4_wo_a_workspace_bytes(int num_tokens, int n_groups, int heads_per_group, int o_lora_rank);
+int b200_dsv4_wo_a(void* stream, const void* o_fp8, const float* o_scale, const void* wo_a, const float* wo_a_scale,
+                   int num_tokens, int n_groups, int heads_per_group, int o_lora_rank, void* workspace,
+                   int64_t workspace_bytes, void* z);
 /* Paged GQA decode.  q [B,Hq,D] bf16, k_cache/v_cache [num_pages,page_size,Hkv,D] bf16 (contiguous), D=128;
  * out bf16 [B,Hq,D], lse f32 [B,Hq] or NULL. */
 int64_t b200_gqa_decode_workspace_bytes(int batch, int num_q_heads, int head_dim, int num_splits);

@@ -88,6 +88,9 @@ PROTOTYPES = {
                                         _i64, _i32, _vp]),
     "b200_dsv4_indices": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _i32, _vp,
                                  _i32]),
+    "b200_dsv4_inv_rope_quant": (_i32, [_vp, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "b200_dsv4_wo_a_workspace_bytes": (_i64, [_i32, _i32, _i32, _i32]),
+    "b200_dsv4_wo_a": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp]),
     "b200_gqa_decode_workspace_bytes": (_i64, [_i32, _i32, _i32, _i32]),
     "b200_gqa_decode": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _f32, _i32,
                                _vp, _vp, _vp]),

@@ -10,7 +10,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libb200moe.so")
-SOURCES = ["api.cu", "moe_prep.cu", "moe_gemm.cu", "moe_fused.cu", "repack.cu", "routing.cu", "router.cu", "attention.cu", "attention_mla.cu", "mla_aux.cu", "attention_gqa.cu", "gqa_aux.cu", "indexer.cu", "ep.cu", "mhc.cu", "dsv4_compress.cu", "dsv4_indices.cu"]
+SOURCES = ["api.cu", "moe_prep.cu", "moe_gemm.cu", "moe_fused.cu", "repack.cu", "routing.cu", "router.cu", "attention.cu", "attention_mla.cu", "mla_aux.cu", "attention_gqa.cu", "gqa_aux.cu", "indexer.cu", "ep.cu", "mhc.cu", "dsv4_compress.cu", "dsv4_indices.cu", "dsv4_oproj.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 

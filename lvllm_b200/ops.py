@@ -1018,3 +1018,103 @@ def dsv4_compressed_slot_mapping(positions: torch.Tensor, slot_mapping: torch.Te
         raise ValueError(f"compress_ratio must be 4 or 128, got {compress_ratio}")
     return _dsv4_indices(_DS_IDX_SLOTMAP, positions, slot_mapping, token_to_req, block_table, block_size, compress_ratio,
                          1)
+
+
+def _dsv4_o_args(o: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.Tensor, n_groups: int):
+    """Checks the attention output and rotary arguments of the V4 output projection; returns (T, H, G, token stride)."""
+    if o.dtype != torch.bfloat16 or o.dim() != 3 or o.shape[2] != 512 or o.stride(2) != 1 \
+            or (o.shape[1] > 1 and o.stride(1) != 512):
+        raise ValueError(f"o must be bf16 [T, H, 512] with contiguous heads and dims, got {o.dtype} {tuple(o.shape)} "
+                         f"strides {o.stride()}")
+    T, H, _ = o.shape
+    G = int(n_groups)
+    if G < 1 or H % G or not 1 <= H // G <= 16:
+        raise ValueError(f"the {H} heads must form n_groups = {n_groups} groups of 1-16 heads")
+    if T > 1 << 20:
+        raise ValueError(f"at most 2^20 tokens, got {T}")
+    stride = o.stride(0) if T > 1 else H * 512
+    if stride < H * 512 or stride % 8 or o.data_ptr() % 16:
+        raise ValueError(f"o's token stride ({o.stride(0)}) must be >= H * 512 and a multiple of 8, its data 16-byte aligned")
+    if cos_sin_cache.dtype != torch.float32 or cos_sin_cache.dim() != 2 or cos_sin_cache.shape[1] != 64 \
+            or cos_sin_cache.shape[0] < 1:
+        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cos_sin_cache.dtype} {tuple(cos_sin_cache.shape)}")
+    if positions.numel() != T:
+        raise ValueError(f"positions needs one entry per token ({T}), got {positions.numel()}")
+    return T, H, G, stride
+
+
+def _dsv4_inv_rope_quant(o, positions, cos_sin_cache, n_groups):
+    T, H, G, stride = _dsv4_o_args(o, positions, cos_sin_cache, n_groups)
+    D = H // G * 512
+    if not o.is_cuda:
+        raise ValueError("o must be a CUDA tensor (lvllm_b200 has no CPU path)")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    cs = _cuda(cos_sin_cache, "cos_sin_cache")
+    o_fp8 = torch.empty(G, T, D, dtype=torch.float8_e4m3fn, device=o.device)
+    o_scale = torch.empty(G, D // 128, T, dtype=torch.float32, device=o.device)
+    rc = L.lib().b200_dsv4_inv_rope_quant(_stream(), o.data_ptr(), stride, pos.data_ptr(), cs.data_ptr(), cs.shape[0], T,
+                                          H, G, o_fp8.data_ptr(), o_scale.data_ptr())
+    L.check(rc, "b200_dsv4_inv_rope_quant")
+    return o_fp8, o_scale
+
+
+def dsv4_inv_rope_quant(o: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.Tensor, n_groups: int):
+    """Inverse RoPE + block-128 fp8 quantisation of the DeepSeek-V4 attention output (the reference's
+    fused_inv_rope_fp8_quant, fp32-scale path, models/deepseek_v4/common/ops/fused_inv_rope_fp8_quant.py).  o bf16
+    [T, H, 512] = [448 nope | 64 rope], heads and dims contiguous, any token stride (a head slice of a padded output);
+    positions [T]; cos_sin_cache f32 [max_pos, 64] = cos | sin (the table ops.dsv4_qnorm_rope_kv_insert takes).  The H heads
+    form n_groups groups of 1-16 heads, D = H / n_groups * 512.  Dims 448-511 of each head get the inverse GPT-J rotation in
+    fp32 (not rounded to bf16); every 128 values of a group get scale 2^ceil(log2(max(absmax, 1e-10) / 448)) and e4m3 codes
+    x / scale, saturating.  Returns (o_fp8 e4m3 [T, n_groups, D], o_scale f32 [T, n_groups, D / 128]), views of
+    group-major storage."""
+    o_fp8, o_scale = _dsv4_inv_rope_quant(o, positions, cos_sin_cache, n_groups)
+    return o_fp8.transpose(0, 1), o_scale.permute(2, 0, 1)
+
+
+_oproj_ws: dict = {}
+_oproj_ws_retired: list = []   # outgrown workspaces stay alive for CUDA graphs captured against them
+
+
+def dsv4_o_proj(o: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.Tensor, wo_a_weight: torch.Tensor,
+                wo_a_scale: torch.Tensor, n_groups: int) -> torch.Tensor:
+    """The DeepSeek-V4 attention output projection up to wo_b (the reference's deep_gemm_fp8_o_proj without its last
+    linear, models/deepseek_v4/nvidia/ops/o_proj.py:28-73): ops.dsv4_inv_rope_quant, then the grouped fp8 GEMM
+    z[t, g, :] = wo_a[g] . o_fp8[t, g, :] (DeepGEMM fp8_einsum("bhr,hdr->bhd"), block-128 scales on both sides).
+    o, positions, cos_sin_cache and n_groups as ops.dsv4_inv_rope_quant.  wo_a_weight e4m3 [n_groups * R, D] and
+    wo_a_scale f32 [n_groups * R / 128, D / 128] are the checkpoint's wo_a, read in place, R = o_lora_rank a multiple of
+    128; checkpoints that store the scales as e8m0 (V4-Flash) convert them to f32 once at load, which is exact.  Each
+    128-wide k-block is one tensor-core accumulation, added in fp32 times both scales.  A token's result does not depend
+    on the other tokens of the call.  Returns z bf16 [T, n_groups * R], the input of wo_b."""
+    T, H, G, _ = _dsv4_o_args(o, positions, cos_sin_cache, n_groups)
+    hpg = H // G
+    D = hpg * 512
+    w, ws = wo_a_weight, wo_a_scale
+    if w.dtype != torch.float8_e4m3fn or w.dim() != 2 or w.shape[1] != D or w.shape[0] % G \
+            or (w.shape[0] // G) % 128 or w.shape[0] == 0:
+        raise ValueError(f"wo_a_weight must be e4m3 [n_groups * R, {D}] with R a multiple of 128, got {w.dtype} "
+                         f"{tuple(w.shape)}")
+    R = w.shape[0] // G
+    if not w.is_contiguous() or w.data_ptr() % 16:
+        raise ValueError("wo_a_weight must be contiguous and 16-byte aligned (it is read in place)")
+    if ws.dtype != torch.float32 or tuple(ws.shape) != (G * R // 128, D // 128):
+        raise ValueError(f"wo_a_scale must be f32 [{G * R // 128}, {D // 128}], got {ws.dtype} {tuple(ws.shape)}")
+    if not (o.is_cuda and w.is_cuda and ws.is_cuda):
+        raise ValueError("o, wo_a_weight and wo_a_scale must be CUDA tensors (lvllm_b200 has no CPU path)")
+    ws = _cuda(ws, "wo_a_scale")
+    z = torch.empty(T, G * R, dtype=torch.bfloat16, device=o.device)
+    if T == 0:
+        return z
+    o_fp8, o_scale = _dsv4_inv_rope_quant(o, positions, cos_sin_cache, G)
+    lib = L.lib()
+    need = int(lib.b200_dsv4_wo_a_workspace_bytes(T, G, hpg, R))
+    key = (o.device.index, torch.cuda.current_stream().cuda_stream)
+    buf = _oproj_ws.get(key)
+    if need and (buf is None or buf.numel() < need):
+        if buf is not None:
+            _oproj_ws_retired.append(buf)
+        buf = torch.zeros(need, dtype=torch.uint8, device=o.device)   # the arrival counters start at zero
+        _oproj_ws[key] = buf
+    rc = lib.b200_dsv4_wo_a(_stream(), o_fp8.data_ptr(), o_scale.data_ptr(), w.data_ptr(), ws.data_ptr(), T, G, hpg, R,
+                            buf.data_ptr() if need else None, buf.numel() if need else 0, z.data_ptr())
+    L.check(rc, "b200_dsv4_wo_a")
+    return z
