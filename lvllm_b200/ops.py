@@ -3,6 +3,10 @@
 Names and argument meaning follow the reference's python op wrappers (vllm/_custom_ops.py ``topk_softmax``,
 ``grouped_topk``, ``moe_permute`` / ``moe_unpermute``, ``sm100_cutlass_mla_decode``) so that parity tests read
 like the reference's own.  All tensors must live on the current CUDA device; there is no CPU path.
+
+The C ABI sees only pointers and sizes, so every op checks the dtype, rank and shape of its tensors here, from metadata
+alone (no value is read: that would synchronise and break CUDA-graph capture), and raises ValueError naming the argument
+before it checks devices, converts or allocates anything.  Limits the C side checks itself are left to it.
 """
 from __future__ import annotations
 
@@ -12,16 +16,23 @@ from . import _lib as L
 
 _DT = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 _OUT = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}
+_ACT = (torch.bfloat16, torch.float16)
+_INT = (torch.int32, torch.int64)
 
 
 def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
-def _cuda(t: torch.Tensor, name: str) -> torch.Tensor:
+def _device(t: torch.Tensor, name: str) -> torch.Tensor:
+    """t itself once it is known to be on a CUDA device: for tensors read or written in place through their strides."""
     if not t.is_cuda:
         raise ValueError(f"{name} must be a CUDA tensor (lvllm_b200 has no CPU path)")
-    return t.contiguous()
+    return t
+
+
+def _cuda(t: torch.Tensor, name: str) -> torch.Tensor:
+    return _device(t, name).contiguous()
 
 
 _SCORING = {"softmax": 0, "sigmoid": 1, "sqrtsoftplus": 2}
@@ -33,14 +44,68 @@ def _i32(t: torch.Tensor, name: str) -> torch.Tensor:
     return t if t.dtype == torch.int32 else t.to(torch.int32)
 
 
+def _per_token(T: int, **index_tensors) -> None:
+    """Each tensor (positions, slot mappings, request rows, ...) must hold one integer per token; None is an absent one."""
+    for name, v in index_tensors.items():
+        if v is not None and (v.dtype not in _INT or v.numel() != T):
+            raise ValueError(f"{name} needs one int32 / int64 entry per token ({T}), got {v.dtype} {tuple(v.shape)}")
+
+
+def _int_tensor(t: torch.Tensor, name: str, dim: int | None = None) -> None:
+    if t.dtype not in _INT or (dim is not None and t.dim() != dim):
+        raise ValueError(f"{name} must be an int32 / int64 tensor{f' of rank {dim}' if dim else ''}, got {t.dtype} "
+                         f"{tuple(t.shape)}")
+
+
+def _cos_sin_cache(cs: torch.Tensor, dtype: torch.dtype = torch.float32) -> None:
+    """The RoPE table [max_pos, 64] = cos | sin that the kernels index by position."""
+    if cs.dtype != dtype or cs.dim() != 2 or cs.shape[1] != 64 or cs.shape[0] < 1:
+        raise ValueError(f"cos_sin_cache must be {dtype} [max_pos, 64], got {cs.dtype} {tuple(cs.shape)}")
+
+
+def _bias(bias: torch.Tensor | None, E: int) -> None:
+    if bias is not None and (not bias.is_floating_point() or bias.numel() != E):
+        raise ValueError(f"e_score_correction_bias must hold one float per expert ({E}), got {bias.dtype} "
+                         f"{tuple(bias.shape)}")
+
+
+def _gating(g: torch.Tensor) -> tuple[int, int]:
+    if g.dtype not in _DT or g.dim() != 2:
+        raise ValueError(f"gating_output must be f32 / bf16 / f16 [tokens, experts], got {g.dtype} {tuple(g.shape)}")
+    return g.shape[0], g.shape[1]
+
+
+def _hash_args(hash_indices_table: torch.Tensor, input_ids: torch.Tensor | None, topk: int, M: int) -> None:
+    if input_ids is None:
+        raise ValueError("hash routing needs input_ids")
+    _int_tensor(hash_indices_table, "hash_indices_table", 2)
+    if hash_indices_table.shape[1] != topk:
+        raise ValueError(f"hash_indices_table must be [vocab, {topk}], got {tuple(hash_indices_table.shape)}")
+    _per_token(M, input_ids=input_ids)
+
+
+_workspaces: dict = {}
+
+
+def _persistent_workspace(kind: str, device: torch.device, nbytes: int) -> torch.Tensor:
+    """A zero-filled byte buffer of at least nbytes, kept per (kind, device, stream) for kernels whose arrival counters
+    must start at zero and that hand them back zeroed.  A larger request replaces the buffer, but the outgrown one stays
+    referenced: a CUDA graph captured against it still writes into it on replay."""
+    bufs = _workspaces.setdefault((kind, device.index, _stream()), [])
+    if not bufs or bufs[-1].numel() < nbytes:
+        bufs.append(torch.zeros(nbytes, dtype=torch.uint8, device=device))
+    return bufs[-1]
+
+
 def fused_topk(gating_output: torch.Tensor, topk: int, renormalize: bool, scoring_func: str = "softmax",
                e_score_correction_bias: torch.Tensor | None = None, routed_scaling_factor: float = 1.0,
                return_token_expert_indices: bool = False):
     """reference fused_topk_router.py:81-124 -> _moe_C.topk_softmax / topk_sigmoid, and fused_topk_bias_router.py ->
     topk_softplus_sqrt for ``scoring_func="sqrtsoftplus"`` (DeepSeek-V4: the bias selects, the weights are the
     unbiased scores)."""
+    M, E = _gating(gating_output)
+    _bias(e_score_correction_bias, E)
     g = _cuda(gating_output, "gating_output")
-    M, E = g.shape
     w = torch.empty(M, topk, dtype=torch.float32, device=g.device)
     ids = torch.empty(M, topk, dtype=torch.int32, device=g.device)
     tei = torch.empty(M, topk, dtype=torch.int32, device=g.device) if return_token_expert_indices else None
@@ -57,13 +122,14 @@ def grouped_topk(gating_output: torch.Tensor, topk: int, renormalize: bool, num_
                  scoring_func: str = "sigmoid", routed_scaling_factor: float = 1.0,
                  e_score_correction_bias: torch.Tensor | None = None):
     """reference grouped_topk_router.py:28-166 (fused kernel semantics: ordered output)."""
+    M, E = _gating(gating_output)
+    _bias(e_score_correction_bias, E)
     g = _cuda(gating_output, "gating_output")
     if scoring_func == "softmax":  # reference applies the softmax in python first (:58-70)
         g = torch.softmax(g.float(), dim=-1)
         scoring = 0
     else:
         scoring = 1
-    M, E = g.shape
     w = torch.empty(M, topk, dtype=torch.float32, device=g.device)
     ids = torch.empty(M, topk, dtype=torch.int32, device=g.device)
     bias = _cuda(e_score_correction_bias.float(), "bias") if e_score_correction_bias is not None else None
@@ -79,23 +145,17 @@ def hash_topk(gating_output: torch.Tensor, topk: int, renormalize: bool, input_i
     """DeepSeek-V4 hash routing (reference topk_softplus_sqrt with ``hash_indices_table``): ids = table[input_ids], in
     table order; weights = sqrt(softplus(logits)) of those experts.  table [vocab, topk]; ids or table entries out of
     range give id -1 and weight 0.  Returns (topk_weights f32 [M,k], topk_ids i32 [M,k])."""
+    M, E = _gating(gating_output)
+    _hash_args(hash_indices_table, input_ids, topk, M)
     g = _cuda(gating_output, "gating_output")
-    M, E = g.shape
     tab = _i32(hash_indices_table, "hash_indices_table")
-    if tab.dim() != 2 or tab.shape[1] != topk:
-        raise ValueError(f"hash_indices_table must be [vocab, {topk}], got {tuple(tab.shape)}")
     ids_in = _i32(input_ids, "input_ids").reshape(-1)
-    if ids_in.numel() != M:
-        raise ValueError(f"input_ids has {ids_in.numel()} tokens, gating_output {M}")
     w = torch.empty(M, topk, dtype=torch.float32, device=g.device)
     ids = torch.empty(M, topk, dtype=torch.int32, device=g.device)
     rc = L.lib().b200_hash_topk(_stream(), g.data_ptr(), _DT[g.dtype], ids_in.data_ptr(), tab.data_ptr(), tab.shape[0], M,
                                 E, topk, int(renormalize), float(routed_scaling_factor), w.data_ptr(), ids.data_ptr())
     L.check(rc, "b200_hash_topk")
     return w, ids
-
-
-_router_ws: dict = {}
 
 
 def router_topk(hidden_states: torch.Tensor, gate_weight: torch.Tensor, topk: int, renormalize: bool,
@@ -113,18 +173,27 @@ def router_topk(hidden_states: torch.Tensor, gate_weight: torch.Tensor, topk: in
     it is V4's hash routing (as ``hash_topk``, on the same kernel's logits).
     Returns (topk_weights f32 [M,k'], topk_ids i32 [M,k'] global, local_ids i32 [M,k'] | None[, logits f32 [M,E]]),
     k' = k + n_shared."""
-    h, wg = _cuda(hidden_states, "hidden_states"), _cuda(gate_weight, "gate_weight")
-    assert h.dtype == wg.dtype and h.dtype in (torch.bfloat16, torch.float16)
+    h, wg = hidden_states, gate_weight
+    if h.dtype not in _ACT or h.dim() != 2:
+        raise ValueError(f"hidden_states must be bf16 / f16 [tokens, hidden], got {h.dtype} {tuple(h.shape)}")
     M, H = h.shape
+    if wg.dtype != h.dtype or wg.dim() != 2 or wg.shape[1] != H:
+        raise ValueError(f"gate_weight must be {h.dtype} [experts, {H}], got {wg.dtype} {tuple(wg.shape)}")
     E = wg.shape[0]
+    _bias(e_score_correction_bias, E)
+    if expert_map is not None:   # the kernel reads expert_map[id] for every id < E
+        _int_tensor(expert_map, "expert_map")
+        if expert_map.numel() < E:
+            raise ValueError(f"expert_map must hold an entry per expert ({E}), got {tuple(expert_map.shape)}")
+    if num_expert_group > 0 and scoring_func not in ("sigmoid", "none"):
+        raise ValueError(f"grouped routing (num_expert_group > 0) scores by sigmoid or none, got {scoring_func!r}")
+    if hash_indices_table is not None:
+        _hash_args(hash_indices_table, input_ids, topk, M)
+    h, wg = _cuda(h, "hidden_states"), _cuda(wg, "gate_weight")
     dev = h.device
     lib = L.lib()
-    need = int(lib.b200_router_workspace_bytes(M, E, H))
-    key = (dev.index, torch.cuda.current_stream().cuda_stream)
-    ws = _router_ws.get(key)
-    if ws is None or ws.numel() < need:
-        ws = torch.zeros(max(need, 1 << 20), dtype=torch.uint8, device=dev)   # counters must start at zero
-        _router_ws[key] = ws
+    # at least 1 MiB: every batch that needs less shares the first buffer
+    ws = _persistent_workspace("router", dev, max(int(lib.b200_router_workspace_bytes(M, E, H)), 1 << 20))
     kk = topk + n_shared
     w = torch.empty(M, kk, dtype=torch.float32, device=dev)
     ids = torch.empty(M, kk, dtype=torch.int32, device=dev)
@@ -133,7 +202,6 @@ def router_topk(hidden_states: torch.Tensor, gate_weight: torch.Tensor, topk: in
     bias = _cuda(e_score_correction_bias.float(), "bias") if e_score_correction_bias is not None else None
     em = _cuda(expert_map.to(torch.int32), "expert_map") if expert_map is not None else None
     if num_expert_group > 0:
-        assert scoring_func in ("sigmoid", "none")
         mode, scoring = 2, 1 if scoring_func == "sigmoid" else 0
     else:
         mode, scoring = {"softmax": 0, "sigmoid": 1, "sqrtsoftplus": 3}[scoring_func], 0
@@ -147,14 +215,8 @@ def router_topk(hidden_states: torch.Tensor, gate_weight: torch.Tensor, topk: in
     if hash_indices_table is None:
         L.check(lib.b200_router_topk(*args), "b200_router_topk")
     else:
-        if input_ids is None:
-            raise ValueError("hash routing needs input_ids")
         tab = _i32(hash_indices_table, "hash_indices_table")
-        if tab.dim() != 2 or tab.shape[1] != topk:
-            raise ValueError(f"hash_indices_table must be [vocab, {topk}], got {tuple(tab.shape)}")
         ids_in = _i32(input_ids, "input_ids").reshape(-1)
-        if ids_in.numel() != M:
-            raise ValueError(f"input_ids has {ids_in.numel()} tokens, hidden_states {M}")
         L.check(lib.b200_router_hash_topk(*args, ids_in.data_ptr(), tab.data_ptr(), tab.shape[0]),
                 "b200_router_hash_topk")
     return (w, ids, loc, lg) if return_logits else (w, ids, loc)
@@ -162,6 +224,8 @@ def router_topk(hidden_states: torch.Tensor, gate_weight: torch.Tensor, topk: in
 
 def global_to_local_expert_ids(topk_ids: torch.Tensor, expert_map: torch.Tensor) -> torch.Tensor:
     """reference routed_experts.py:1332-1342."""
+    _int_tensor(topk_ids, "topk_ids")
+    _int_tensor(expert_map, "expert_map")
     ids = _cuda(topk_ids.to(torch.int32), "topk_ids")
     em = _cuda(expert_map.to(torch.int32), "expert_map")
     out = torch.empty_like(ids)
@@ -173,8 +237,13 @@ def global_to_local_expert_ids(topk_ids: torch.Tensor, expert_map: torch.Tensor)
 def moe_permute(hidden_states: torch.Tensor | None, topk_ids: torch.Tensor, n_local_expert: int):
     """Stable sort by expert (reference moe_permute_unpermute.py:105-231).  Returns
     (permuted_hidden | None, sorted_slot i32 [M*k], expert_first_token_offset i64 [E+1], inv_permuted_idx i32 [M,k])."""
+    _int_tensor(topk_ids, "topk_ids", 2)
+    M, k = topk_ids.shape
+    if hidden_states is not None and (hidden_states.dtype not in _ACT or hidden_states.dim() != 2
+                                      or hidden_states.shape[0] != M):
+        raise ValueError(f"hidden_states must be bf16 / f16 [{M}, hidden] (a row per token of topk_ids), got "
+                         f"{hidden_states.dtype} {tuple(hidden_states.shape)}")
     ids = _cuda(topk_ids.to(torch.int32), "topk_ids")
-    M, k = ids.shape
     dev = ids.device
     sorted_slot = torch.empty(M * k, dtype=torch.int32, device=dev)
     first = torch.empty(n_local_expert + 1, dtype=torch.int64, device=dev)
@@ -183,7 +252,6 @@ def moe_permute(hidden_states: torch.Tensor | None, topk_ids: torch.Tensor, n_lo
     hp, H = None, 0
     if hidden_states is not None:
         h = _cuda(hidden_states, "hidden_states")
-        assert h.dtype in (torch.bfloat16, torch.float16)
         H = h.shape[1]
         perm = torch.zeros(M * k, H, dtype=h.dtype, device=dev)
         hp = h.data_ptr()
@@ -196,12 +264,20 @@ def moe_permute(hidden_states: torch.Tensor | None, topk_ids: torch.Tensor, n_lo
 def moe_unpermute(permuted: torch.Tensor, topk_weights: torch.Tensor, inv_permuted_idx: torch.Tensor,
                   out_dtype: torch.dtype | None = None) -> torch.Tensor:
     """out[t] = sum_j w[t,j] * permuted[inv[t,j]] in fp32 (reference moe_permute_unpermute.py:234-277)."""
+    if permuted.dtype not in _ACT or permuted.dim() != 2:
+        raise ValueError(f"permuted must be bf16 / f16 [rows, hidden], got {permuted.dtype} {tuple(permuted.shape)}")
+    _int_tensor(inv_permuted_idx, "inv_permuted_idx", 2)
+    if not topk_weights.is_floating_point() or topk_weights.shape != inv_permuted_idx.shape:
+        raise ValueError(f"topk_weights must be float {tuple(inv_permuted_idx.shape)} like inv_permuted_idx, got "
+                         f"{topk_weights.dtype} {tuple(topk_weights.shape)}")
+    od = out_dtype or permuted.dtype
+    if od not in _OUT:
+        raise ValueError(f"out_dtype must be bf16, f16 or f32, got {od}")
     p = _cuda(permuted, "permuted")
     w = _cuda(topk_weights.float(), "topk_weights")
     inv = _cuda(inv_permuted_idx.to(torch.int32), "inv_permuted_idx")
     M, k = inv.shape
     H = p.shape[1]
-    od = out_dtype or p.dtype
     out = torch.empty(M, H, dtype=od, device=p.device)
     rc = L.lib().b200_moe_unpermute(_stream(), p.data_ptr(), 1 if p.dtype == torch.float16 else 0, w.data_ptr(),
                                     inv.data_ptr(), M, k, H, out.data_ptr(), _OUT[od])
@@ -212,8 +288,13 @@ def moe_unpermute(permuted: torch.Tensor, topk_weights: torch.Tensor, inv_permut
 def rmsnorm_cast(x_f32: torch.Tensor, out: torch.Tensor, gain: float = 1.0, eps: float = 1e-6) -> torch.Tensor:
     """out = cast(x * gain * rsqrt(mean(x^2)+eps)) — the cast Lvllm applies to lk_moe's fp32 output
     (reference routed_experts.py:1855) fused with the RMS normalisation that follows in the layer."""
+    if x_f32.dtype != torch.float32 or x_f32.dim() != 2:
+        raise ValueError(f"x must be f32 [tokens, hidden], got {x_f32.dtype} {tuple(x_f32.shape)}")
+    if out.dtype not in _ACT or out.shape != x_f32.shape or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous bf16 / f16 {tuple(x_f32.shape)} tensor, got {out.dtype} "
+                         f"{tuple(out.shape)}")
     x = _cuda(x_f32, "x")
-    assert x.dtype == torch.float32 and out.is_cuda and out.is_contiguous()
+    _device(out, "out")
     M, H = x.shape
     L.check(L.lib().b200_rmsnorm_cast(_stream(), x.data_ptr(), out.data_ptr(), M, H, float(gain), float(eps),
                                       1 if out.dtype == torch.float16 else 0), "b200_rmsnorm_cast")
@@ -226,6 +307,22 @@ def _mla_splits(max_keys: int, rows: int) -> int:
     softmax; rows = grid rows (requests x q-groups, or query tokens).  Enough splits to fill ~2 waves of the 132 SMs, no
     more: each split costs an fp32 partial of the output."""
     return max(1, min(-(-max_keys // 128), 264 // (4 * rows)))
+
+
+def _mla_queries(q_nope: torch.Tensor, q_pe: torch.Tensor, dtypes: tuple) -> tuple[int, int]:
+    """Checks the absorbed MLA query halves q_nope [T, Hq, 512] / q_pe [T, Hq, 64] of one dtype; returns (T, Hq)."""
+    if q_nope.dtype not in dtypes or q_nope.dim() != 3 or q_nope.shape[2] != 512:
+        raise ValueError(f"q_nope must be {' / '.join(map(str, dtypes))} [tokens, heads, 512], got {q_nope.dtype} "
+                         f"{tuple(q_nope.shape)}")
+    T, Hq, _ = q_nope.shape
+    if q_pe.dtype != q_nope.dtype or tuple(q_pe.shape) != (T, Hq, 64):
+        raise ValueError(f"q_pe must be {q_nope.dtype} [{T}, {Hq}, 64], got {q_pe.dtype} {tuple(q_pe.shape)}")
+    return T, Hq
+
+
+def _w_uv(w_uv: torch.Tensor | None, Hq: int) -> None:
+    if w_uv is not None and (w_uv.dtype != torch.bfloat16 or tuple(w_uv.shape) != (Hq, 512, 128)):
+        raise ValueError(f"w_uv must be bf16 [{Hq}, 512, 128], got {w_uv.dtype} {tuple(w_uv.shape)}")
 
 
 def mla_decode(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_c_and_k_pe_cache: torch.Tensor, seq_lens: torch.Tensor,
@@ -243,22 +340,26 @@ def mla_decode(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_c_and_k_pe_cache: to
     single-token decode.
     With ``w_uv`` [Hq,512,128] the split merge is fused with the v up-projection and (out_v [B*Q,Hq,128], out, lse) is
     returned.  Returns (out bf16 [B*Q,Hq,512], lse f32 [B*Q,Hq])."""
-    qn, qp = _cuda(q_nope, "q_nope"), _cuda(q_pe, "q_pe")
-    kv = _cuda(kv_c_and_k_pe_cache, "kv_cache")
     f8 = torch.float8_e4m3fn
-    assert kv.dtype in (torch.bfloat16, f8) and kv.shape[-1] == 576
-    assert qn.dtype == qp.dtype and qn.dtype in (torch.bfloat16, f8) and (qn.dtype != f8 or kv.dtype == f8)
-    T, Hq, _ = qn.shape
+    kv = kv_c_and_k_pe_cache
+    if kv.dtype not in (torch.bfloat16, f8) or kv.dim() != 3 or kv.shape[2] != 576:
+        raise ValueError(f"kv_cache must be bf16 or e4m3 [pages, page, 576], got {kv.dtype} {tuple(kv.shape)}")
+    T, Hq = _mla_queries(q_nope, q_pe, (torch.bfloat16, f8) if kv.dtype == f8 else (torch.bfloat16,))
+    _int_tensor(seq_lens, "seq_lens")
+    _int_tensor(page_table, "page_table", 2)
     Q = int(q_len_per_req)
+    B = seq_lens.numel()
+    if T != B * Q:
+        raise ValueError(f"q_nope / q_pe must hold q_len_per_req = {Q} tokens per request: {B * Q} rows for {B} seq_lens, "
+                         f"got {T}")
+    if page_table.shape[0] < B:   # the kernel reads row b of the table for every request b < B
+        raise ValueError(f"page_table must have a row per request ({B}), got {tuple(page_table.shape)}")
+    _w_uv(w_uv, Hq)
+    qn, qp = _cuda(q_nope, "q_nope"), _cuda(q_pe, "q_pe")
+    kv = _cuda(kv, "kv_cache")
     page = kv.shape[1]
     sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
     pt = _cuda(page_table.to(torch.int32), "page_table")
-    B = sl.numel()
-    if T != B * Q or qp.shape[0] != T:
-        raise ValueError(f"q_nope / q_pe must hold q_len_per_req = {Q} tokens per request: {B * Q} rows for {B} seq_lens, "
-                         f"got {T} / {qp.shape[0]}")
-    if pt.dim() != 2 or pt.shape[0] < B:   # the kernel reads row b of the table for every request b < B
-        raise ValueError(f"page_table must have a row per request ({B}), got {tuple(pt.shape)}")
     max_pages = pt.shape[1]
     if max_seq_len is not None:
         # the kernel only walks pages below the bound: a narrower view of the table keeps the split count (and the
@@ -278,7 +379,6 @@ def mla_decode(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_c_and_k_pe_cache: to
     if w_uv is not None:
         # split merge fused with the v up-projection (reference _v_up_proj, mla_attention.py:1154-1176)
         wv = _cuda(w_uv, "w_uv")
-        assert wv.dtype == torch.bfloat16 and wv.shape == (Hq, 512, 128)
         out_v = torch.empty(T, Hq, 128, dtype=torch.bfloat16, device=qn.device)
         L.check(L.lib().b200_mla_decode_spec(*args, wv.data_ptr(), out_v.data_ptr()), "b200_mla_decode_vup")
         return out_v, out, lse
@@ -297,21 +397,23 @@ def mla_decode_sparse(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_cache: torch.
     req_id [T]; page_table [R, max_pages].  A token with no valid entry gets out 0 and lse -inf.
     With ``w_uv`` [Hq,512,128] the split merge is fused with the v up-projection and (out_v [T,Hq,128], out, lse) is
     returned.  Returns (out bf16 [T,Hq,512], lse f32 [T,Hq])."""
+    if q_nope.dtype != torch.bfloat16 or q_pe.dtype != torch.bfloat16:
+        raise ValueError(f"sparse MLA decode takes bf16 queries, got {q_nope.dtype} / {q_pe.dtype}")
+    if kv_cache.dim() != 3 or (kv_cache.dtype, kv_cache.shape[-1]) not in ((torch.bfloat16, 576), (torch.uint8, 656)):
+        raise ValueError(f"kv_cache must be bf16 [pages, page, 576] or fp8_ds_mla uint8 [pages, page, 656], "
+                         f"got {kv_cache.dtype} {tuple(kv_cache.shape)}")
+    T, Hq = _mla_queries(q_nope, q_pe, (torch.bfloat16,))
+    _int_tensor(topk_indices, "topk_indices", 2)
+    if topk_indices.shape[0] != T:
+        raise ValueError(f"topk_indices needs one row per query token ({T}), got {tuple(topk_indices.shape)}")
+    _per_token(T, req_id=req_id)
+    _int_tensor(page_table, "page_table", 2)
+    _w_uv(w_uv, Hq)
     qn, qp = _cuda(q_nope, "q_nope"), _cuda(q_pe, "q_pe")
     kv = _cuda(kv_cache, "kv_cache")
-    if qn.dtype != torch.bfloat16 or qp.dtype != torch.bfloat16:
-        raise ValueError(f"sparse MLA decode takes bf16 queries, got {qn.dtype} / {qp.dtype}")
-    if kv.dim() != 3 or (kv.dtype, kv.shape[-1]) not in ((torch.bfloat16, 576), (torch.uint8, 656)):
-        raise ValueError(f"kv_cache must be bf16 [pages, page, 576] or fp8_ds_mla uint8 [pages, page, 656], "
-                         f"got {kv.dtype} {tuple(kv.shape)}")
-    T, Hq, _ = qn.shape
     idx = _cuda(topk_indices.to(torch.int32), "topk_indices")
     rid = _cuda(req_id.reshape(-1).to(torch.int32), "req_id")
     pt = _cuda(page_table.to(torch.int32), "page_table")
-    if idx.dim() != 2 or idx.shape[0] != T or rid.numel() != T or qp.shape[0] != T:
-        raise ValueError(f"q_pe, topk_indices and req_id need one row per query token ({T})")
-    if pt.dim() != 2:
-        raise ValueError(f"page_table must be [requests, max_pages], got {tuple(pt.shape)}")
     topk = idx.shape[1]
     if num_kv_splits <= 0:
         num_kv_splits = _mla_splits(topk, T)
@@ -323,7 +425,6 @@ def mla_decode_sparse(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_cache: torch.
             out.data_ptr(), lse.data_ptr()]
     if w_uv is not None:
         wv = _cuda(w_uv, "w_uv")
-        assert wv.dtype == torch.bfloat16 and wv.shape == (Hq, 512, 128)
         out_v = torch.empty(T, Hq, 128, dtype=torch.bfloat16, device=qn.device)
         L.check(L.lib().b200_mla_decode_sparse(*args, wv.data_ptr(), out_v.data_ptr()), "b200_mla_decode_sparse")
         return out_v, out, lse
@@ -332,14 +433,12 @@ def mla_decode_sparse(q_nope: torch.Tensor, q_pe: torch.Tensor, kv_cache: torch.
 
 
 def _dsv4_cache(c: torch.Tensor, name: str):
-    """(tensor, block_size, num_blocks, block stride in bytes) of a 584-byte-per-token cache, uint8 [blocks, block_size, 584];
+    """(block_size, num_blocks, block stride in bytes) of a 584-byte-per-token cache, uint8 [blocks, block_size, 584];
     blocks may be padded (stride(0) > block_size * 584), the bytes of a block are addressed as the per-block layout."""
-    if not c.is_cuda:
-        raise ValueError(f"{name} must be a CUDA tensor (lvllm_b200 has no CPU path)")
     if c.dtype != torch.uint8 or c.dim() != 3 or c.shape[2] != 584 or c.stride(2) != 1 or c.stride(1) != 584:
         raise ValueError(f"{name} must be uint8 [blocks, block_size, 584] with rows of 584 contiguous bytes, "
                          f"got {c.dtype} {tuple(c.shape)} strides {c.stride()}")
-    return c, c.shape[1], c.shape[0], c.stride(0)
+    return c.shape[1], c.shape[0], c.stride(0)
 
 
 def dsv4_sparse_decode(q: torch.Tensor, swa_cache: torch.Tensor, swa_indices: torch.Tensor, swa_lens: torch.Tensor,
@@ -353,35 +452,36 @@ def dsv4_sparse_decode(q: torch.Tensor, swa_cache: torch.Tensor, swa_indices: to
     extra_indices[t, :extra_lens[t]] (global slots of extra_cache, compressed layers only); a slot < 0 or past its cache is
     no key.  One cache row is both key and value.  attn_sink f32 [Hq] adds e^(sink) to each head's softmax denominator.
     A token with no valid key gets out 0.  Returns out bf16 [T, Hq, 512]."""
-    q = _cuda(q, "q")
     if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 512:
         raise ValueError(f"q must be bf16 [tokens, heads, 512], got {q.dtype} {tuple(q.shape)}")
     T, Hq, _ = q.shape
     if not 1 <= Hq <= 128 or not 1 <= T <= 65535:
         raise ValueError(f"dsv4 sparse decode takes 1-128 heads and 1-65535 tokens, got {Hq} heads, {T} tokens")
-    sc, sbs, snb, sstride = _dsv4_cache(swa_cache, "swa_cache")
+    sbs, snb, sstride = _dsv4_cache(swa_cache, "swa_cache")
 
-    def _lists(idx, lens, name):
-        idx = _cuda(idx.to(torch.int32), f"{name}_indices")
-        lens = _cuda(lens.reshape(-1).to(torch.int32), f"{name}_lens")
-        if idx.dim() != 2 or idx.shape[0] != T or idx.shape[1] < 1 or lens.numel() != T:
-            raise ValueError(f"{name}_indices must be [{T}, topk >= 1] and {name}_lens [{T}], got {tuple(idx.shape)} / "
-                             f"{tuple(lens.shape)}")
-        return idx, lens
+    def _check_lists(idx, lens, name):
+        if idx.dtype not in _INT or idx.dim() != 2 or idx.shape[0] != T or idx.shape[1] < 1:
+            raise ValueError(f"{name}_indices must be int [{T}, topk >= 1], got {idx.dtype} {tuple(idx.shape)}")
+        _per_token(T, **{f"{name}_lens": lens})
 
-    si, sl = _lists(swa_indices, swa_lens, "swa")
+    _check_lists(swa_indices, swa_lens, "swa")
     if (extra_cache is None) != (extra_indices is None) or (extra_indices is None) != (extra_lens is None):
         raise ValueError("extra_cache, extra_indices and extra_lens go together")
     if extra_cache is not None:
-        ec, ebs, enb, estride = _dsv4_cache(extra_cache, "extra_cache")
-        ei, el = _lists(extra_indices, extra_lens, "extra")
+        ebs, enb, estride = _dsv4_cache(extra_cache, "extra_cache")
+        _check_lists(extra_indices, extra_lens, "extra")
     else:
-        ec, ebs, enb, estride, ei, el = None, 0, 0, 0, None, None
-    sink = None
-    if attn_sink is not None:
-        sink = _cuda(attn_sink.reshape(-1).to(torch.float32), "attn_sink")
-        if sink.numel() != Hq:
-            raise ValueError(f"attn_sink must hold one value per head ({Hq}), got {sink.numel()}")
+        ebs, enb, estride = 0, 0, 0
+    if attn_sink is not None and (not attn_sink.is_floating_point() or attn_sink.numel() != Hq):
+        raise ValueError(f"attn_sink must hold one float per head ({Hq}), got {attn_sink.dtype} {tuple(attn_sink.shape)}")
+    q = _cuda(q, "q")
+    sc = _device(swa_cache, "swa_cache")
+    si, sl = _i32(swa_indices, "swa_indices"), _i32(swa_lens.reshape(-1), "swa_lens")
+    ec, ei, el = None, None, None
+    if extra_cache is not None:
+        ec = _device(extra_cache, "extra_cache")
+        ei, el = _i32(extra_indices, "extra_indices"), _i32(extra_lens.reshape(-1), "extra_lens")
+    sink = _cuda(attn_sink.reshape(-1).to(torch.float32), "attn_sink") if attn_sink is not None else None
     if num_kv_splits <= 0:
         num_kv_splits = _mla_splits(si.shape[1] + (ei.shape[1] if ei is not None else 0), T)
     ws = torch.empty(L.lib().b200_mla_decode_workspace_bytes(T, Hq, num_kv_splits), dtype=torch.uint8, device=q.device)
@@ -404,7 +504,6 @@ def dsv4_qnorm_rope_kv_insert(q: torch.Tensor, kv: torch.Tensor, positions: torc
     dims are quantised per 64 to e4m3 with a ue8m0 scale, and the row goes to slot_mapping[t] of swa_cache (uint8
     [blocks, block_size, 584]; a slot < 0 writes nothing).  positions int64 [T]; cos_sin_cache f32 [max_pos, 64] = cos | sin.
     Returns q_out bf16 [T, q_head_padded, 512], heads past Hq zero."""
-    q, kv = _cuda(q, "q"), _cuda(kv, "kv")
     if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 512:
         raise ValueError(f"q must be bf16 [tokens, heads, 512], got {q.dtype} {tuple(q.shape)}")
     T, Hq, _ = q.shape
@@ -412,14 +511,14 @@ def dsv4_qnorm_rope_kv_insert(q: torch.Tensor, kv: torch.Tensor, positions: torc
         raise ValueError(f"kv must be bf16 [{T}, 512], got {kv.dtype} {tuple(kv.shape)}")
     if int(q_head_padded) < Hq:
         raise ValueError(f"q_head_padded ({q_head_padded}) must be >= the head count ({Hq})")
+    _cos_sin_cache(cos_sin_cache)
+    _per_token(T, positions=positions, slot_mapping=slot_mapping)
+    bs, nb, stride = _dsv4_cache(swa_cache, "swa_cache")
+    q, kv = _cuda(q, "q"), _cuda(kv, "kv")
     cs = _cuda(cos_sin_cache, "cos_sin_cache")
-    if cs.dtype != torch.float32 or cs.dim() != 2 or cs.shape[1] != 64:
-        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cs.dtype} {tuple(cs.shape)}")
     pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
     slots = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
-    if pos.numel() != T or slots.numel() != T:
-        raise ValueError(f"positions and slot_mapping need one entry per token ({T})")
-    c, bs, nb, stride = _dsv4_cache(swa_cache, "swa_cache")
+    c = _device(swa_cache, "swa_cache")
     q_out = torch.empty(T, int(q_head_padded), 512, dtype=torch.bfloat16, device=q.device)
     rc = L.lib().b200_dsv4_qnorm_rope_kv_insert(_stream(), q.data_ptr(), kv.data_ptr(), pos.data_ptr(), cs.data_ptr(),
                                                 cs.shape[0], slots.data_ptr(), c.data_ptr(), bs, nb, stride, q_out.data_ptr(),
@@ -464,20 +563,16 @@ def dsv4_compress(kv_score: torch.Tensor, ape: torch.Tensor, positions: torch.Te
             or state_cache.stride(2) != 1 or state_cache.stride(1) != 2 * half:
         raise ValueError(f"state_cache must be f32 [blocks, block_size, {2 * half}] with contiguous rows, got "
                          f"{state_cache.dtype} {tuple(state_cache.shape)} strides {state_cache.stride()}")
-    if block_table.dim() != 2 or block_table.stride(1) != 1 or block_table.dtype not in (torch.int32, torch.int64):
+    if block_table.dim() != 2 or block_table.stride(1) != 1 or block_table.dtype not in _INT:
         raise ValueError(f"block_table must be int [requests, max_blocks] with contiguous rows, got {block_table.dtype} "
                          f"{tuple(block_table.shape)}")
-    if cos_sin_cache.dtype != torch.float32 or cos_sin_cache.dim() != 2 or cos_sin_cache.shape[1] != 64:
-        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cos_sin_cache.dtype} {tuple(cos_sin_cache.shape)}")
-    for name, v in (("positions", positions), ("slot_mapping", slot_mapping), ("token_to_req", token_to_req),
-                    ("kv_slot_mapping", kv_slot_mapping)):
-        if v.numel() != T:
-            raise ValueError(f"{name} needs one entry per token ({T}), got {v.numel()}")
+    _cos_sin_cache(cos_sin_cache)
+    _per_token(T, positions=positions, slot_mapping=slot_mapping, token_to_req=token_to_req,
+               kv_slot_mapping=kv_slot_mapping)
     if T == 0:
         return
-    ks, sc, kc = kv_score, state_cache, kv_cache   # written or read in place, through their strides
-    if not ks.is_cuda or not sc.is_cuda or not kc.is_cuda:
-        raise ValueError("kv_score, state_cache and kv_cache must be CUDA tensors (lvllm_b200 has no CPU path)")
+    # written or read in place, through their strides
+    ks, sc, kc = _device(kv_score, "kv_score"), _device(state_cache, "state_cache"), _device(kv_cache, "kv_cache")
     w, cs, ap = _cuda(norm_weight, "norm_weight"), _cuda(cos_sin_cache, "cos_sin_cache"), _cuda(ape, "ape")
     bt = _i32(block_table, "block_table")
     pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
@@ -492,38 +587,46 @@ def dsv4_compress(kv_score: torch.Tensor, ape: torch.Tensor, positions: torch.Te
 
 
 def _mhc_streams(residual: torch.Tensor, name: str = "residual"):
-    """bf16 [..., 4, H] -> (contiguous tensor, leading shape, T, H)."""
-    r = _cuda(residual, name)
+    """bf16 [..., 4, H] -> (leading shape, T, H)."""
+    r = residual
     if r.dtype != torch.bfloat16 or r.dim() < 2 or r.shape[-2] != 4:
         raise ValueError(f"{name} must be bf16 [..., 4, hidden] (hc_mult = 4), got {r.dtype} {tuple(r.shape)}")
-    lead = tuple(r.shape[:-2])
-    return r, lead, r.numel() // (4 * r.shape[-1]) if r.numel() else 0, r.shape[-1]
+    return tuple(r.shape[:-2]), r.numel() // (4 * r.shape[-1]) if r.numel() else 0, r.shape[-1]
 
 
-def _mhc_f32(t: torch.Tensor, numel: int, name: str) -> torch.Tensor:
-    t = _cuda(t.to(torch.float32), name)
-    if t.numel() != numel:
-        raise ValueError(f"{name} must hold {numel} float32 values, got shape {tuple(t.shape)}")
-    return t
+def _mhc_f32(t: torch.Tensor, numel: int, name: str) -> None:
+    if not t.is_floating_point() or t.numel() != numel:
+        raise ValueError(f"{name} must hold {numel} float32 values, got {t.dtype} {tuple(t.shape)}")
+
+
+def _mhc_x(x: torch.Tensor, T: int, H: int) -> None:
+    if x.dtype != torch.bfloat16 or x.numel() != T * H:
+        raise ValueError(f"x must be bf16 [..., {H}] with the residual's leading shape, got {x.dtype} {tuple(x.shape)}")
+
+
+def _f32(t: torch.Tensor, name: str) -> torch.Tensor:
+    return _cuda(t.to(torch.float32), name)
 
 
 def _mhc_post_pre(x, residual, post_layer_mix, comb_res_mix, fn, hc_scale, hc_base, rms_eps, hc_pre_eps, hc_sinkhorn_eps,
                   hc_post_mult_value, sinkhorn_repeat, norm_weight, norm_eps):
-    r, lead, T, H = _mhc_streams(residual)
-    fn = _mhc_f32(fn, 24 * 4 * H, "fn")
-    sc, base = _mhc_f32(hc_scale, 3, "hc_scale"), _mhc_f32(hc_base, 24, "hc_base")
+    lead, T, H = _mhc_streams(residual)
+    _mhc_f32(fn, 24 * 4 * H, "fn")
+    _mhc_f32(hc_scale, 3, "hc_scale")
+    _mhc_f32(hc_base, 24, "hc_base")
     post = x is not None
     if post:
+        _mhc_x(x, T, H)
+        _mhc_f32(post_layer_mix, T * 4, "post_layer_mix")
+        _mhc_f32(comb_res_mix, T * 16, "comb_res_mix")
+    if norm_weight is not None and (not norm_weight.is_floating_point() or norm_weight.numel() != H):
+        raise ValueError(f"norm_weight must hold {H} values, got {norm_weight.dtype} {tuple(norm_weight.shape)}")
+    r = _cuda(residual, "residual")
+    fn, sc, base = _f32(fn, "fn"), _f32(hc_scale, "hc_scale"), _f32(hc_base, "hc_base")
+    if post:
         x = _cuda(x, "x")
-        if x.dtype != torch.bfloat16 or x.numel() != T * H:
-            raise ValueError(f"x must be bf16 [..., {H}] with the residual's leading shape, got {x.dtype} {tuple(x.shape)}")
-        plm = _mhc_f32(post_layer_mix, T * 4, "post_layer_mix")
-        crm = _mhc_f32(comb_res_mix, T * 16, "comb_res_mix")
-    w = None
-    if norm_weight is not None:
-        w = _cuda(norm_weight.to(torch.bfloat16), "norm_weight")
-        if w.numel() != H:
-            raise ValueError(f"norm_weight must hold {H} values, got shape {tuple(norm_weight.shape)}")
+        plm, crm = _f32(post_layer_mix, "post_layer_mix"), _f32(comb_res_mix, "comb_res_mix")
+    w = _cuda(norm_weight.to(torch.bfloat16), "norm_weight") if norm_weight is not None else None
     dev = r.device
     r_out = torch.empty_like(r) if post else None
     post_mix = torch.empty(*lead, 4, 1, dtype=torch.float32, device=dev)
@@ -561,12 +664,12 @@ def mhc_post(x: torch.Tensor, residual: torch.Tensor, post_layer_mix: torch.Tens
     """DeepSeek-V4 mHC post mapping (the reference's mhc_post_tilelang; torch.py:94-106): x bf16 [..., H], residual bf16
     [..., 4, H], post_layer_mix f32 [..., 4] or [..., 4, 1], comb_res_mix f32 [..., 4, 4];
     out[..., j, :] = bf16(post[j] x + sum_i comb[i, j] residual[i]) in fp32.  Returns bf16 [..., 4, H]."""
-    r, lead, T, H = _mhc_streams(residual)
-    x = _cuda(x, "x")
-    if x.dtype != torch.bfloat16 or x.numel() != T * H:
-        raise ValueError(f"x must be bf16 [..., {H}] with the residual's leading shape, got {x.dtype} {tuple(x.shape)}")
-    plm = _mhc_f32(post_layer_mix, T * 4, "post_layer_mix")
-    crm = _mhc_f32(comb_res_mix, T * 16, "comb_res_mix")
+    _, T, H = _mhc_streams(residual)
+    _mhc_x(x, T, H)
+    _mhc_f32(post_layer_mix, T * 4, "post_layer_mix")
+    _mhc_f32(comb_res_mix, T * 16, "comb_res_mix")
+    r, x = _cuda(residual, "residual"), _cuda(x, "x")
+    plm, crm = _f32(post_layer_mix, "post_layer_mix"), _f32(comb_res_mix, "comb_res_mix")
     out = torch.empty_like(r)
     if T:
         rc = L.lib().b200_mhc_post(_stream(), x.data_ptr(), r.data_ptr(), plm.data_ptr(), crm.data_ptr(), T, H, out.data_ptr())
@@ -591,9 +694,12 @@ def hc_head(hidden_states: torch.Tensor, hc_fn: torch.Tensor, hc_scale: torch.Te
     """DeepSeek-V4 hc_head (the reference's hc_head_fused_kernel_tilelang): collapses the 4 streams before the final norm.
     hidden_states bf16 [T, 4, H], hc_fn f32 [4, 4H], hc_scale f32 [1], hc_base f32 [4];
     out = bf16(sum_i (sigmoid(mix_i * rsqrt(mean(r_flat^2) + rms_norm_eps) * s + base_i) + hc_eps) r_i).  Returns bf16 [T, H]."""
-    r, lead, T, H = _mhc_streams(hidden_states, "hidden_states")
-    fn = _mhc_f32(hc_fn, 4 * 4 * H, "hc_fn")
-    sc, base = _mhc_f32(hc_scale, 1, "hc_scale"), _mhc_f32(hc_base, 4, "hc_base")
+    lead, T, H = _mhc_streams(hidden_states, "hidden_states")
+    _mhc_f32(hc_fn, 4 * 4 * H, "hc_fn")
+    _mhc_f32(hc_scale, 1, "hc_scale")
+    _mhc_f32(hc_base, 4, "hc_base")
+    r = _cuda(hidden_states, "hidden_states")
+    fn, sc, base = _f32(hc_fn, "hc_fn"), _f32(hc_scale, "hc_scale"), _f32(hc_base, "hc_base")
     out = torch.empty(*lead, H, dtype=torch.bfloat16, device=r.device)
     if T:
         ws = torch.empty(L.lib().b200_mhc_workspace_bytes(T, H), dtype=torch.uint8, device=r.device)
@@ -610,26 +716,40 @@ def mla_rope_cache_write(q_pe: torch.Tensor, k_pe: torch.Tensor, kv_c: torch.Ten
     concat_and_cache_mla: kv_cache [blocks, block_size, 576] (bf16 or e4m3) row slot_mapping[t] <- [kv_c[t] | rope(k_pe[t])].
     A uint8 [blocks, block_size, 656] cache is the fp8_ds_mla layout of concat_and_cache_ds_mla_kernel (per-128-dim fp32
     scales, bf16 rope part; kv_scale is not used)."""
-    for t, n in ((q_pe, "q_pe"), (k_pe, "k_pe"), (kv_c, "kv_c"), (cos_sin_cache, "cos_sin_cache")):
-        assert t.is_cuda and t.is_contiguous() and t.dtype == torch.bfloat16, n
-    ds_mla = kv_cache.dtype == torch.uint8 and kv_cache.shape[-1] == 656
-    assert kv_cache.is_cuda and kv_cache.is_contiguous() and (ds_mla or kv_cache.shape[-1] == 576)
-    assert cos_sin_cache.shape[-1] == 64
+    if q_pe.dtype != torch.bfloat16 or q_pe.dim() != 3 or q_pe.shape[2] != 64 or not q_pe.is_contiguous():
+        raise ValueError(f"q_pe must be a contiguous bf16 [tokens, heads, 64] tensor (rotated in place), got {q_pe.dtype} "
+                         f"{tuple(q_pe.shape)}")
     T, Hq, _ = q_pe.shape
-    pos = _cuda(positions.to(torch.int64), "positions")
-    sm = _cuda(slot_mapping.to(torch.int64), "slot_mapping")
+    if k_pe.dtype != torch.bfloat16 or tuple(k_pe.shape) != (T, 64) or not k_pe.is_contiguous():
+        raise ValueError(f"k_pe must be a contiguous bf16 [{T}, 64] tensor (rotated in place), got {k_pe.dtype} "
+                         f"{tuple(k_pe.shape)}")
+    if kv_c.dtype != torch.bfloat16 or tuple(kv_c.shape) != (T, 512):
+        raise ValueError(f"kv_c must be bf16 [{T}, 512], got {kv_c.dtype} {tuple(kv_c.shape)}")
+    _cos_sin_cache(cos_sin_cache, torch.bfloat16)
+    _per_token(T, positions=positions, slot_mapping=slot_mapping)
+    if kv_cache.dim() != 3 or not kv_cache.is_contiguous() or (kv_cache.dtype, kv_cache.shape[2]) not in (
+            (torch.bfloat16, 576), (torch.float8_e4m3fn, 576), (torch.uint8, 656)):
+        raise ValueError(f"kv_cache must be a contiguous bf16 / e4m3 [blocks, block_size, 576] or uint8 "
+                         f"[blocks, block_size, 656] tensor, got {kv_cache.dtype} {tuple(kv_cache.shape)}")
+    q_pe, k_pe, kv_cache = _device(q_pe, "q_pe"), _device(k_pe, "k_pe"), _device(kv_cache, "kv_cache")
+    kv_c, cs = _cuda(kv_c, "kv_c"), _cuda(cos_sin_cache, "cos_sin_cache")
+    pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
+    sm = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
+    kv_dtype = {torch.bfloat16: 0, torch.float8_e4m3fn: 1, torch.uint8: 2}[kv_cache.dtype]
     rc = L.lib().b200_mla_rope_cache_write(_stream(), q_pe.data_ptr(), k_pe.data_ptr(), kv_c.data_ptr(), pos.data_ptr(),
-                                           cos_sin_cache.data_ptr(), int(is_neox_style), sm.data_ptr(), kv_cache.data_ptr(),
-                                           2 if ds_mla else int(kv_cache.dtype == torch.float8_e4m3fn), float(kv_scale),
-                                           T, Hq)
+                                           cs.data_ptr(), int(is_neox_style), sm.data_ptr(), kv_cache.data_ptr(), kv_dtype,
+                                           float(kv_scale), T, Hq)
     L.check(rc, "b200_mla_rope_cache_write")
 
 
 def mla_q_absorb(q_nope: torch.Tensor, w_uk_t: torch.Tensor) -> torch.Tensor:
     """ql_nope [T,Hq,512] = q_nope [T,Hq,128] x W_UK_T [Hq,128,512] (reference mla_attention.py:875-893)."""
+    if q_nope.dtype != torch.bfloat16 or q_nope.dim() != 3 or q_nope.shape[2] != 128:
+        raise ValueError(f"q_nope must be bf16 [tokens, heads, 128], got {q_nope.dtype} {tuple(q_nope.shape)}")
+    T, Hq, _ = q_nope.shape
+    if w_uk_t.dtype != torch.bfloat16 or tuple(w_uk_t.shape) != (Hq, 128, 512):
+        raise ValueError(f"w_uk_t must be bf16 [{Hq}, 128, 512], got {w_uk_t.dtype} {tuple(w_uk_t.shape)}")
     q, w = _cuda(q_nope, "q_nope"), _cuda(w_uk_t, "w_uk_t")
-    T, Hq, P = q.shape
-    assert q.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and P == 128 and w.shape == (Hq, 128, 512)
     out = torch.empty(T, Hq, 512, dtype=torch.bfloat16, device=q.device)
     L.check(L.lib().b200_mla_q_absorb(_stream(), q.data_ptr(), w.data_ptr(), out.data_ptr(), T, Hq), "b200_mla_q_absorb")
     return out
@@ -640,8 +760,6 @@ def _kv_cache_strides(k_cache: torch.Tensor, v_cache: torch.Tensor) -> tuple[int
     the kernels address: the FlashInfer backend's packed NHD / HND halves (kv_cache.transpose(1, 2).split(128, -1),
     flashinfer.py:2276-2290) or separate contiguous caches.  Never copies: a write through a copy would be lost."""
     for t, n in ((k_cache, "k_cache"), (v_cache, "v_cache")):
-        if not t.is_cuda:
-            raise ValueError(f"{n} must be a CUDA tensor (lvllm_b200 has no CPU path)")
         if t.dtype != torch.bfloat16 or t.dim() != 4 or t.shape[-1] != 128:
             raise ValueError(f"{n} must be a bf16 [blocks, page, num_kv_heads, 128] view, got {t.dtype} {tuple(t.shape)}")
     if k_cache.shape != v_cache.shape or k_cache.stride() != v_cache.stride() or k_cache.device != v_cache.device:
@@ -666,19 +784,23 @@ def gqa_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, se
     .split(128, -1)); the head dim must be contiguous and the other strides multiples of 8 elements (ValueError otherwise).
     ``max_seq_len`` (host-side bound on seq_lens, as the reference's attention metadata carries it) sizes the split count
     and the B*Hq*splits*130*4-byte workspace from the real context instead of the page-table width (= max_model_len)."""
-    qq = _cuda(q, "q")
-    assert qq.dtype == torch.bfloat16
     bstride, pstride, hstride = _kv_cache_strides(k_cache, v_cache)
-    T, Hq, D = qq.shape
+    if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 128:
+        raise ValueError(f"q must be bf16 [tokens, heads, 128], got {q.dtype} {tuple(q.shape)}")
+    T, Hq, D = q.shape
     Q = int(q_len_per_req)
     page, Hkv = k_cache.shape[1], k_cache.shape[2]
-    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
-    pt = _cuda(page_table.to(torch.int32), "page_table")
-    B = sl.numel()
+    _int_tensor(seq_lens, "seq_lens")
+    _int_tensor(page_table, "page_table", 2)
+    B = seq_lens.numel()
     if T != B * Q:
         raise ValueError(f"q must hold q_len_per_req = {Q} tokens per request: {B * Q} rows for {B} seq_lens, got {T}")
-    if pt.dim() != 2 or pt.shape[0] != B:
-        raise ValueError(f"page_table must have one row per request ({B}), got {tuple(pt.shape)}")
+    if page_table.shape[0] != B:
+        raise ValueError(f"page_table must have one row per request ({B}), got {tuple(page_table.shape)}")
+    qq = _cuda(q, "q")
+    k_cache, v_cache = _device(k_cache, "k_cache"), _device(v_cache, "v_cache")
+    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
+    pt = _cuda(page_table.to(torch.int32), "page_table")
     if max_seq_len is not None:
         max_pages = max(1, min(pt.shape[1], -(-int(max_seq_len) // page)))
         if max_pages != pt.shape[1]:
@@ -710,27 +832,25 @@ def gqa_qknorm_rope_cache_write(qkv: torch.Tensor, positions: torch.Tensor, cos_
     cos_sin_cache bf16 [max_position, rotary_dim] = cos | sin; slot_mapping [T] (< 0: padded token, nothing written);
     k_cache / v_cache the views exactly as the reference passes them to reshape_and_cache_flash.
     Returns q_out [T, Hq, 128] bf16, contiguous: the q that gqa_decode takes."""
-    x = _cuda(qkv, "qkv")
+    x = qkv
     if x.dtype != torch.bfloat16 or x.dim() != 2 or x.shape[1] != (num_heads + 2 * num_kv_heads) * 128:
         raise ValueError(f"qkv must be bf16 [T, (num_heads + 2 * num_kv_heads) * 128], got {x.dtype} {tuple(x.shape)}")
-    cs = _cuda(cos_sin_cache, "cos_sin_cache")
-    if cs.dtype != torch.bfloat16 or cs.dim() != 2:
+    if cos_sin_cache.dtype != torch.bfloat16 or cos_sin_cache.dim() != 2:
         raise ValueError("cos_sin_cache must be bf16 [max_position, rotary_dim]")
     bstride, pstride, hstride = _kv_cache_strides(k_cache, v_cache)
     if k_cache.shape[2] != num_kv_heads or k_cache.device != x.device:
         raise ValueError("the cache views must hold num_kv_heads heads on qkv's device")
-    ws = []
     for w, n in ((q_norm_weight, "q_norm_weight"), (k_norm_weight, "k_norm_weight")):
-        if w is not None:
-            w = _cuda(w, n)
-            if w.dtype != torch.bfloat16 or w.numel() != 128:
-                raise ValueError(f"{n} must be bf16 [128]")
-        ws.append(w)
+        if w is not None and (w.dtype != torch.bfloat16 or w.numel() != 128):
+            raise ValueError(f"{n} must be bf16 [128]")
     T = x.shape[0]
+    _per_token(T, positions=positions, slot_mapping=slot_mapping)
+    x = _cuda(x, "qkv")
+    cs = _cuda(cos_sin_cache, "cos_sin_cache")
+    ws = [_cuda(w, n) if w is not None else None for w, n in ((q_norm_weight, "q_norm_weight"),
+                                                               (k_norm_weight, "k_norm_weight"))]
     pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
     sm = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
-    if pos.numel() != T or sm.numel() != T:
-        raise ValueError("positions and slot_mapping need one entry per token")
     q_out = torch.empty(T, num_heads, 128, dtype=torch.bfloat16, device=x.device)
     rc = L.lib().b200_gqa_qknorm_rope_cache_write(
         _stream(), x.data_ptr(), pos.data_ptr(), cs.data_ptr(), cs.shape[0], cs.shape[1], int(is_neox_style),
@@ -739,6 +859,19 @@ def gqa_qknorm_rope_cache_write(qkv: torch.Tensor, positions: torch.Tensor, cos_
         q_out.data_ptr(), T, num_heads, num_kv_heads, 128)
     L.check(rc, "b200_gqa_qknorm_rope_cache_write")
     return q_out
+
+
+def _weights_view(weights: torch.Tensor, T: int, H: int) -> None:
+    """The indexer weights, bf16 [T, H] read through their row stride (a column slice of the fused projection)."""
+    if weights.dtype != torch.bfloat16 or weights.shape != (T, H) or weights.stride(1) != 1 \
+            or (T > 1 and weights.stride(0) < H):
+        raise ValueError(f"weights must be a bf16 [{T}, {H}] view with contiguous, non-overlapping rows")
+
+
+def _indexer_cache(k_cache: torch.Tensor) -> None:
+    if k_cache.dtype != torch.uint8 or k_cache.dim() != 3 or k_cache.shape[2] != 132 or not k_cache.is_contiguous():
+        raise ValueError(f"k_cache must be a contiguous uint8 [num_blocks, block_size, 132], got {k_cache.dtype} "
+                         f"{tuple(k_cache.shape)}")
 
 
 def indexer_qk_rope_quant_cache_write(q: torch.Tensor, weights: torch.Tensor, k: torch.Tensor, positions: torch.Tensor,
@@ -751,26 +884,20 @@ def indexer_qk_rope_quant_cache_write(q: torch.Tensor, weights: torch.Tensor, k:
     (a column slice of the fused projection); k [T,128] bf16 after k_norm; cos_sin_cache bf16 [max_position, 64];
     slot_mapping [T] (< 0: nothing written); k_cache uint8 [num_blocks, block_size, 132], written in place.
     Returns (q_fp8 e4m3 [T,H,128], weights_out f32 [T,H] = weight * q_scale * softmax_scale * head_scale)."""
-    x = _cuda(q, "q")
-    kk = _cuda(k, "k")
-    if x.dtype != torch.bfloat16 or x.dim() != 3 or x.shape[2] != 128:
-        raise ValueError(f"q must be bf16 [T, H, 128], got {x.dtype} {tuple(x.shape)}")
-    T, H, _ = x.shape
-    if kk.dtype != torch.bfloat16 or kk.shape != (T, 128):
-        raise ValueError(f"k must be bf16 [{T}, 128], got {kk.dtype} {tuple(kk.shape)}")
-    if not weights.is_cuda or weights.dtype != torch.bfloat16 or weights.shape != (T, H) or weights.stride(1) != 1 \
-            or (T > 1 and weights.stride(0) < H):
-        raise ValueError(f"weights must be a bf16 [{T}, {H}] view with contiguous, non-overlapping rows")
+    if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 128:
+        raise ValueError(f"q must be bf16 [T, H, 128], got {q.dtype} {tuple(q.shape)}")
+    T, H, _ = q.shape
+    if k.dtype != torch.bfloat16 or k.shape != (T, 128):
+        raise ValueError(f"k must be bf16 [{T}, 128], got {k.dtype} {tuple(k.shape)}")
+    _weights_view(weights, T, H)
+    _cos_sin_cache(cos_sin_cache, torch.bfloat16)
+    _indexer_cache(k_cache)
+    _per_token(T, positions=positions, slot_mapping=slot_mapping)
+    x, kk = _cuda(q, "q"), _cuda(k, "k")
+    weights, k_cache = _device(weights, "weights"), _device(k_cache, "k_cache")
     cs = _cuda(cos_sin_cache, "cos_sin_cache")
-    if cs.dtype != torch.bfloat16 or cs.dim() != 2 or cs.shape[1] != 64:
-        raise ValueError("cos_sin_cache must be bf16 [max_position, 64]")
-    if not k_cache.is_cuda or k_cache.dtype != torch.uint8 or k_cache.dim() != 3 or k_cache.shape[2] != 132 \
-            or not k_cache.is_contiguous():
-        raise ValueError(f"k_cache must be a contiguous uint8 [num_blocks, block_size, 132], got {tuple(k_cache.shape)}")
     pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
     sm = _cuda(slot_mapping.reshape(-1).to(torch.int64), "slot_mapping")
-    if pos.numel() != T or sm.numel() != T:
-        raise ValueError("positions and slot_mapping need one entry per token")
     q_fp8 = torch.empty(T, H, 128, dtype=torch.float8_e4m3fn, device=x.device)
     w_out = torch.empty(T, H, dtype=torch.float32, device=x.device)
     rc = L.lib().b200_indexer_qk_rope_quant_cache_write(
@@ -781,11 +908,10 @@ def indexer_qk_rope_quant_cache_write(q: torch.Tensor, weights: torch.Tensor, k:
     return q_fp8, w_out
 
 
-def _indexer_cache(k_cache: torch.Tensor) -> torch.Tensor:
-    if not k_cache.is_cuda or k_cache.dtype != torch.uint8 or k_cache.dim() != 3 or k_cache.shape[2] != 132 \
-            or not k_cache.is_contiguous():
-        raise ValueError(f"k_cache must be a contiguous uint8 [num_blocks, block_size, 132], got {tuple(k_cache.shape)}")
-    return k_cache
+def _logits_out(logits: torch.Tensor, R: int, width: int) -> None:
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.shape[0] != R or logits.shape[1] < width \
+            or logits.stride(1) != 1:
+        raise ValueError(f"logits must be f32 [{R}, >= {width}] with contiguous rows")
 
 
 def indexer_logits(q_fp8: torch.Tensor, weights: torch.Tensor, k_cache: torch.Tensor, seq_lens: torch.Tensor,
@@ -795,26 +921,26 @@ def indexer_logits(q_fp8: torch.Tensor, weights: torch.Tensor, k_cache: torch.Te
     j <= seq_lens[b] - Q + i; -inf to the end of the request's last page, the rest untouched.  q_fp8 [B*Q,H,128] e4m3,
     weights f32 [B*Q,H]; H 32 or 64, Q <= 16, page 16 / 32 / 64.  ``logits`` (f32 [B*Q, >= max_pages * page]) is filled
     in place when given.  Returns logits."""
-    q8 = _cuda(q_fp8, "q_fp8")
-    w = _cuda(weights, "weights")
-    kc = _indexer_cache(k_cache)
-    if q8.dtype != torch.float8_e4m3fn or q8.dim() != 3 or q8.shape[2] != 128:
-        raise ValueError(f"q_fp8 must be e4m3 [B*Q, H, 128], got {q8.dtype} {tuple(q8.shape)}")
-    R, H, _ = q8.shape
-    if w.dtype != torch.float32 or w.shape != (R, H):
+    if q_fp8.dtype != torch.float8_e4m3fn or q_fp8.dim() != 3 or q_fp8.shape[2] != 128:
+        raise ValueError(f"q_fp8 must be e4m3 [B*Q, H, 128], got {q_fp8.dtype} {tuple(q_fp8.shape)}")
+    R, H, _ = q_fp8.shape
+    if weights.dtype != torch.float32 or weights.shape != (R, H):
         raise ValueError(f"weights must be f32 [{R}, {H}]")
+    _indexer_cache(k_cache)
+    _int_tensor(seq_lens, "seq_lens")
+    _int_tensor(page_table, "page_table", 2)
+    B, Q = seq_lens.numel(), int(q_len)
+    if R != B * Q or page_table.shape[0] < B:
+        raise ValueError(f"q_fp8 needs q_len = {Q} rows per request ({B * Q}), page_table a row per request")
+    page = k_cache.shape[1]
+    width = page_table.shape[1] * page
+    if logits is not None:
+        _logits_out(logits, R, width)
+    q8, w, kc = _cuda(q_fp8, "q_fp8"), _cuda(weights, "weights"), _device(k_cache, "k_cache")
     sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
     pt = _cuda(page_table.to(torch.int32), "page_table")
-    B, Q = sl.numel(), int(q_len)
-    if R != B * Q or pt.dim() != 2 or pt.shape[0] < B:
-        raise ValueError(f"q_fp8 needs q_len = {Q} rows per request ({B * Q}), page_table a row per request")
-    page = kc.shape[1]
-    width = pt.shape[1] * page
-    if logits is None:
-        logits = torch.empty(R, width, dtype=torch.float32, device=q8.device)
-    elif logits.dtype != torch.float32 or logits.dim() != 2 or logits.shape[0] != R or logits.shape[1] < width \
-            or logits.stride(1) != 1:
-        raise ValueError(f"logits must be f32 [{R}, >= {width}] with contiguous rows")
+    logits = _device(logits, "logits") if logits is not None else torch.empty(R, width, dtype=torch.float32,
+                                                                              device=q8.device)
     rc = L.lib().b200_indexer_logits(_stream(), q8.data_ptr(), w.data_ptr(), kc.data_ptr(), kc.shape[0], page,
                                      sl.data_ptr(), pt.data_ptr(), B, Q, H, pt.shape[1], logits.data_ptr(),
                                      logits.stride(0))
@@ -828,13 +954,14 @@ def indexer_topk(logits: torch.Tensor, seq_lens: torch.Tensor, topk: int, q_len:
     -1 padding.  ``logits`` may be a column slice of a wider buffer (rows read through its own row stride).
     Returns int32 [B*Q, topk]."""
     lg = logits
-    if not lg.is_cuda or lg.dtype != torch.float32 or lg.dim() != 2 or lg.stride(1) != 1 \
-            or (lg.shape[0] > 1 and lg.stride(0) < lg.shape[1]):
-        raise ValueError("logits must be a CUDA f32 [rows, width] tensor with contiguous, non-overlapping rows")
-    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
-    B, Q = sl.numel(), int(q_len)
+    if lg.dtype != torch.float32 or lg.dim() != 2 or lg.stride(1) != 1 or (lg.shape[0] > 1 and lg.stride(0) < lg.shape[1]):
+        raise ValueError("logits must be an f32 [rows, width] tensor with contiguous, non-overlapping rows")
+    _int_tensor(seq_lens, "seq_lens")
+    B, Q = seq_lens.numel(), int(q_len)
     if lg.shape[0] != B * Q:
         raise ValueError(f"logits needs q_len = {Q} rows per request ({B * Q}), got {lg.shape[0]}")
+    lg = _device(lg, "logits")
+    sl = _cuda(seq_lens.reshape(-1).to(torch.int32), "seq_lens")
     out = torch.empty(B * Q, int(topk), dtype=torch.int32, device=lg.device)
     row_stride = lg.stride(0) if lg.shape[0] > 1 else lg.shape[1]
     rc = L.lib().b200_indexer_topk(_stream(), lg.data_ptr(), row_stride, lg.shape[1], sl.data_ptr(), B, Q, int(topk),
@@ -863,16 +990,10 @@ def dsv4_indexer_q_quant(q: torch.Tensor, weights: torch.Tensor, positions: torc
     if q.dtype != torch.bfloat16 or q.dim() != 3 or q.shape[2] != 128 or not 1 <= q.shape[1] <= 128:
         raise ValueError(f"q must be bf16 [T, 1-128 heads, 128], got {q.dtype} {tuple(q.shape)}")
     T, H, _ = q.shape
-    if weights.dtype != torch.bfloat16 or weights.shape != (T, H) or weights.stride(1) != 1 \
-            or (T > 1 and weights.stride(0) < H):
-        raise ValueError(f"weights must be a bf16 [{T}, {H}] view with contiguous, non-overlapping rows")
-    if cos_sin_cache.dtype != torch.float32 or cos_sin_cache.dim() != 2 or cos_sin_cache.shape[1] != 64:
-        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cos_sin_cache.dtype} "
-                         f"{tuple(cos_sin_cache.shape)}")
-    if positions.numel() != T:
-        raise ValueError(f"positions needs one entry per token ({T}), got {positions.numel()}")
-    if not weights.is_cuda:
-        raise ValueError("weights must be a CUDA tensor (lvllm_b200 has no CPU path)")
+    _weights_view(weights, T, H)
+    _cos_sin_cache(cos_sin_cache)
+    _per_token(T, positions=positions)
+    weights = _device(weights, "weights")
     x, cs = _cuda(q, "q"), _cuda(cos_sin_cache, "cos_sin_cache")
     pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
     q_fp8 = torch.empty(T, H, 128, dtype=torch.float8_e4m3fn, device=x.device)
@@ -900,30 +1021,27 @@ def dsv4_indexer_decode(q_fp8: torch.Tensor, weights: torch.Tensor, k_cache: tor
     T, H, _ = q_fp8.shape
     if weights.dtype != torch.float32 or weights.shape != (T, H):
         raise ValueError(f"weights must be f32 [{T}, {H}], got {weights.dtype} {tuple(weights.shape)}")
-    if k_cache.dtype != torch.uint8 or k_cache.dim() != 3 or k_cache.shape[2] != 132 or not k_cache.is_contiguous():
-        raise ValueError(f"k_cache must be a contiguous uint8 [num_blocks, page, 132], got {tuple(k_cache.shape)}")
-    if block_table.dim() != 2 or block_table.dtype not in (torch.int32, torch.int64):
+    _indexer_cache(k_cache)
+    if block_table.dim() != 2 or block_table.dtype not in _INT:
         raise ValueError(f"block_table must be int [requests, max_blocks], got {block_table.dtype} "
                          f"{tuple(block_table.shape)}")
     ratio, k = int(compress_ratio), int(topk)
     if ratio not in (4, 128) or not 1 <= k <= 2048:
         raise ValueError(f"compress_ratio must be 4 or 128 and topk 1-2048, got {ratio}, {k}")
-    if positions.numel() != T or token_to_req.numel() != T:
-        raise ValueError(f"positions and token_to_req need one entry per token ({T})")
+    _per_token(T, positions=positions, token_to_req=token_to_req)
     page = k_cache.shape[1]
     width = block_table.shape[1] * page
-    if logits is None:
-        logits = torch.empty(T, width, dtype=torch.float32, device=q_fp8.device)
-    elif logits.dtype != torch.float32 or logits.dim() != 2 or logits.shape[0] != T or logits.shape[1] < width \
-            or logits.stride(1) != 1:
-        raise ValueError(f"logits must be f32 [{T}, >= {width}] with contiguous rows")
-    out = torch.empty(T, k, dtype=torch.int32, device=q_fp8.device)
+    if logits is not None:
+        _logits_out(logits, T, width)
     if T == 0:
-        return out
-    q8, w, kc = _cuda(q_fp8, "q_fp8"), _cuda(weights, "weights"), _cuda(k_cache, "k_cache")
+        return torch.empty(T, k, dtype=torch.int32, device=q_fp8.device)
+    q8, w, kc = _cuda(q_fp8, "q_fp8"), _cuda(weights, "weights"), _device(k_cache, "k_cache")
     pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
     req = _i32(token_to_req.reshape(-1), "token_to_req")
     bt = _i32(block_table, "block_table")
+    logits = _device(logits, "logits") if logits is not None else torch.empty(T, width, dtype=torch.float32,
+                                                                              device=q8.device)
+    out = torch.empty(T, k, dtype=torch.int32, device=q8.device)
     rc = L.lib().b200_dsv4_indexer_decode(
         _stream(), q8.data_ptr(), w.data_ptr(), kc.data_ptr(), kc.shape[0], page, pos.data_ptr(), req.data_ptr(),
         bt.data_ptr(), bt.shape[1], ratio, T, H, int(max_seq_len) if max_seq_len is not None else 0, logits.data_ptr(),
@@ -938,15 +1056,13 @@ _DS_IDX_SWA, _DS_IDX_C128A, _DS_IDX_TOPK, _DS_IDX_SLOTMAP = 0, 1, 2, 3
 def _dsv4_indices(kind: int, positions, slot_mapping, token_to_req, block_table, block_size: int, param: int,
                   width: int, local_topk=None):
     """One b200_dsv4_indices call; returns (indices int32 [T, width], lens int32 [T]), or the int64 [T] slot mapping."""
-    if block_table.dim() != 2 or block_table.dtype not in (torch.int32, torch.int64) or block_table.shape[1] < 1:
+    if block_table.dim() != 2 or block_table.dtype not in _INT or block_table.shape[1] < 1:
         raise ValueError(f"block_table must be int [requests, max_blocks >= 1], got {block_table.dtype} "
                          f"{tuple(block_table.shape)}")
     if int(block_size) < 1:
         raise ValueError(f"block_size must be >= 1, got {block_size}")
     T = positions.numel() if local_topk is None else local_topk.shape[0]
-    for name, v in (("positions", positions), ("slot_mapping", slot_mapping), ("token_to_req", token_to_req)):
-        if v is not None and v.numel() != T:
-            raise ValueError(f"{name} needs one entry per token ({T}), got {v.numel()}")
+    _per_token(T, positions=positions, slot_mapping=slot_mapping, token_to_req=token_to_req)
     dev = block_table.device
     if kind == _DS_IDX_SLOTMAP:
         out, lens = torch.empty(T, dtype=torch.int64, device=dev), None
@@ -1000,7 +1116,7 @@ def dsv4_global_topk_indices(topk_indices: torch.Tensor, slot_mapping: torch.Ten
     block_table[token_to_req[t]][i // block_size] * block_size + i % block_size (a block column >= max_blocks: -1), -1
     stays -1; the length is the count of entries >= 0, 0 for a token with slot_mapping < 0.
     Returns (extra_indices int32 [T, topk]; extra_lens int32 [T])."""
-    if topk_indices.dim() != 2 or topk_indices.dtype not in (torch.int32, torch.int64) or topk_indices.shape[1] < 1:
+    if topk_indices.dim() != 2 or topk_indices.dtype not in _INT or topk_indices.shape[1] < 1:
         raise ValueError(f"topk_indices must be int [tokens, topk >= 1], got {topk_indices.dtype} "
                          f"{tuple(topk_indices.shape)}")
     return _dsv4_indices(_DS_IDX_TOPK, None, slot_mapping, token_to_req, block_table, block_size, 0,
@@ -1035,19 +1151,15 @@ def _dsv4_o_args(o: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.
     stride = o.stride(0) if T > 1 else H * 512
     if stride < H * 512 or stride % 8 or o.data_ptr() % 16:
         raise ValueError(f"o's token stride ({o.stride(0)}) must be >= H * 512 and a multiple of 8, its data 16-byte aligned")
-    if cos_sin_cache.dtype != torch.float32 or cos_sin_cache.dim() != 2 or cos_sin_cache.shape[1] != 64 \
-            or cos_sin_cache.shape[0] < 1:
-        raise ValueError(f"cos_sin_cache must be f32 [max_pos, 64], got {cos_sin_cache.dtype} {tuple(cos_sin_cache.shape)}")
-    if positions.numel() != T:
-        raise ValueError(f"positions needs one entry per token ({T}), got {positions.numel()}")
+    _cos_sin_cache(cos_sin_cache)
+    _per_token(T, positions=positions)
     return T, H, G, stride
 
 
 def _dsv4_inv_rope_quant(o, positions, cos_sin_cache, n_groups):
     T, H, G, stride = _dsv4_o_args(o, positions, cos_sin_cache, n_groups)
     D = H // G * 512
-    if not o.is_cuda:
-        raise ValueError("o must be a CUDA tensor (lvllm_b200 has no CPU path)")
+    o = _device(o, "o")
     pos = _cuda(positions.reshape(-1).to(torch.int64), "positions")
     cs = _cuda(cos_sin_cache, "cos_sin_cache")
     o_fp8 = torch.empty(G, T, D, dtype=torch.float8_e4m3fn, device=o.device)
@@ -1069,10 +1181,6 @@ def dsv4_inv_rope_quant(o: torch.Tensor, positions: torch.Tensor, cos_sin_cache:
     group-major storage."""
     o_fp8, o_scale = _dsv4_inv_rope_quant(o, positions, cos_sin_cache, n_groups)
     return o_fp8.transpose(0, 1), o_scale.permute(2, 0, 1)
-
-
-_oproj_ws: dict = {}
-_oproj_ws_retired: list = []   # outgrown workspaces stay alive for CUDA graphs captured against them
 
 
 def dsv4_o_proj(o: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.Tensor, wo_a_weight: torch.Tensor,
@@ -1098,22 +1206,15 @@ def dsv4_o_proj(o: torch.Tensor, positions: torch.Tensor, cos_sin_cache: torch.T
         raise ValueError("wo_a_weight must be contiguous and 16-byte aligned (it is read in place)")
     if ws.dtype != torch.float32 or tuple(ws.shape) != (G * R // 128, D // 128):
         raise ValueError(f"wo_a_scale must be f32 [{G * R // 128}, {D // 128}], got {ws.dtype} {tuple(ws.shape)}")
-    if not (o.is_cuda and w.is_cuda and ws.is_cuda):
-        raise ValueError("o, wo_a_weight and wo_a_scale must be CUDA tensors (lvllm_b200 has no CPU path)")
-    ws = _cuda(ws, "wo_a_scale")
+    _device(o, "o")
+    w, ws = _device(w, "wo_a_weight"), _cuda(ws, "wo_a_scale")
     z = torch.empty(T, G * R, dtype=torch.bfloat16, device=o.device)
     if T == 0:
         return z
     o_fp8, o_scale = _dsv4_inv_rope_quant(o, positions, cos_sin_cache, G)
     lib = L.lib()
     need = int(lib.b200_dsv4_wo_a_workspace_bytes(T, G, hpg, R))
-    key = (o.device.index, torch.cuda.current_stream().cuda_stream)
-    buf = _oproj_ws.get(key)
-    if need and (buf is None or buf.numel() < need):
-        if buf is not None:
-            _oproj_ws_retired.append(buf)
-        buf = torch.zeros(need, dtype=torch.uint8, device=o.device)   # the arrival counters start at zero
-        _oproj_ws[key] = buf
+    buf = _persistent_workspace("dsv4_wo_a", o.device, need) if need else None
     rc = lib.b200_dsv4_wo_a(_stream(), o_fp8.data_ptr(), o_scale.data_ptr(), w.data_ptr(), ws.data_ptr(), T, G, hpg, R,
                             buf.data_ptr() if need else None, buf.numel() if need else 0, z.data_ptr())
     L.check(rc, "b200_dsv4_wo_a")
